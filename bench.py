@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — frames/sec of the latent-walk hot path (BASELINE.json metric) on N B200s.
+"""bench.py — frames/sec of the latent-walk hot path (BASELINE.json metric) on N H100s.
 
   python bench.py --gpus 1 --steps K --warmup W             native arm (libsdwalk.so)
   python bench.py --impl reference ...                       the reference's CPU path (oracle restatement), rank 0
   torchrun --nproc-per-node N bench.py --gpus N ...          one rank per GPU, frames sharded, NCCL gather
+  python bench.py ... --dump-outputs DIR                     also write the last timed step's frames to DIR/*.npy
 
 Workload (config.workload): BASELINE.json configs[1] — SD-1.4 architecture, 512x512, fp16, PNDM 50 steps
 (51 UNet calls), classifier-free guidance 7.5, frames interpolated between 2 synthetic prompts; random-init weights
@@ -22,38 +23,26 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the kernels the roofline block names, taken from committed
-# `ncu --set full` captures (profiles/roofline_traffic.json: bytes, the batch of the capture, the raw page they come from)
-def _traffic(kernel, batch):
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "roofline_traffic.json")))[kernel]
-        return {"bytes": t["bytes"] * batch / t["batch"], "source": f"ncu capture {t['source']} at batch {t['batch']}, "
-                                                                   f"scaled to batch {batch}"}
-    except Exception:
-        return {"bytes": None, "source": "no capture committed"}
-
-
 FLOP_PER_FRAME = {"sd14": 2 * 51 * 0.8033e12 + 2.5145e12}  # SURVEY.md §8d algorithmic FLOPs (84.45 T)
 UNET_FLOP_B1 = 0.8033e12
 VAE_FLOP = 2.5145e12
 
 
-def _peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1440.7), d.get("hbm_gbs", 6564.5), "measured"
-    return 1400.0, 6650.0, "fallback"
+# NVIDIA's H100 SXM data sheet (700 W card): dense fp16 / bf16 tensor TFLOP/s and HBM3 GB/s.  A card set to a lower power
+# limit reaches less; the run reports its power limit and clocks beside the fractions.
+H100_FP16_TFLOPS = 989.4
+H100_HBM_GBS = 3350.0
+DUMP_MAX_ELEMS = 12 << 20  # float32 elements written by --dump-outputs (48 MB)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / power / throttle reasons sampled (read-only queries) DURING the timed region."""
 
     def __init__(self, index):
         self.rows, self.proc, self.index = [], None, index
 
     def start(self):
-        q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
+        q = ("clocks.sm,clocks.max.sm,power.draw,power.limit,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
              "clocks_event_reasons.sw_power_cap")
         try:
@@ -74,12 +63,13 @@ class ClockSampler:
         reasons = set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
-            for n, v in zip(names, r[3:7]):
+            for n, v in zip(names, r[4:8]):
                 if v.lower().startswith("active"):
                     reasons.add(n)
         mx = max((int(float(r[1])) for r in self.rows if len(r) > 1 and r[1].replace(".", "").isdigit()), default=0)
-        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx or None, "reasons": sorted(reasons),
-                "samples": len(sm)}
+        pl = [float(r[3]) for r in self.rows if len(r) > 3 and r[3].replace(".", "").isdigit()]
+        return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx or None, "power_limit_w": pl[0] if pl else None,
+                "reasons": sorted(reasons), "samples": len(sm)}
 
 
 def cpu_reference_leg(steps, warmup, budget_s=150.0):
@@ -93,8 +83,7 @@ def cpu_reference_leg(steps, warmup, budget_s=150.0):
     from oracle.vae import AutoencoderKLDecoder, VAEConfig
 
     # BASELINE.md §3: all host cores, whatever OMP_NUM_THREADS the launcher exported (torchrun sets it to 1).  "All cores" =
-    # the PHYSICAL cores this process may run on: with one thread per hyper-thread (os.cpu_count() = 128 on the GPU box) the
-    # same forward took 88 s instead of 7.6 s (profiles/r02_bench_F30_db_attention.json vs BENCH_r01)
+    # the PHYSICAL cores this process may run on: one thread per hyper-thread makes the CPU forward many times slower
     try:
         import psutil
 
@@ -171,6 +160,9 @@ def main():
     ap.add_argument("--inference-steps", type=int, default=50)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (its uint8 frames as float32) to "
+                         "DIR/frames.npy; above 48 MB a fixed seeded sample of the flattened frames, in index order")
     a = ap.parse_args()
     saved_stdout = _stdout_to_stderr()
 
@@ -254,7 +246,7 @@ def main():
         lat, emb = batch(i)
         u8 = eng.sample(lat, emb, unc, use_graph=not a.no_graph)
         if world > 1 and gather:
-            gather_frames(u8, F * world)  # decoded frames to rank 0 over NCCL
+            u8 = gather_frames(u8, F * world)  # decoded frames to rank 0 over NCCL
         return u8
 
     for i in range(W):
@@ -266,11 +258,20 @@ def main():
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     ev0.record()
+    last = None
     for i in range(K):
-        run_step(W + i)
+        last = run_step(W + i)
     ev1.record()
     barrier()
     ms = ev0.elapsed_time(ev1)
+    if a.dump_outputs and rank == 0 and last is not None:
+        import numpy as np
+
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        frames = last.cpu().numpy().astype(np.float32).reshape(-1)
+        if frames.size > DUMP_MAX_ELEMS:
+            frames = frames[np.sort(np.random.default_rng(0).choice(frames.size, DUMP_MAX_ELEMS, replace=False))]
+        np.save(os.path.join(a.dump_outputs, "frames.npy"), frames)
     if world > 1:
         tt = torch.tensor([ms], device=dev)
         dist.all_reduce(tt, op=dist.ReduceOp.MAX)
@@ -328,7 +329,7 @@ def main():
         import ctypes as C
 
         Bn = 2 * F
-        flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > 126 MB L2
+        flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)  # > the 50 MB L2
 
         def timed(fn, warm=2, reps=6):
             for _ in range(warm):
@@ -370,7 +371,7 @@ def main():
         d.bias = bk.data_ptr(); d.resid = rk.data_ptr(); d.ldr = 320
         d.out = ok.data_ptr(); d.ldc = 320; d.alpha = 1.0
         conv_us = timed(lambda: _native.gemm(d))
-        kern = {"name": "gemm2_tc_kernel<160, tap-reuse> conv3x3 64x64 320->320 bias+residual", "batch": Bn,
+        kern = {"name": "gemm_kernel (CTA pairs, tap reuse) conv3x3 64x64 320->320 bias+residual", "batch": Bn,
                 "flop_per_launch": 2.0 * Bn * 64 * 64 * 320 * 2880, "us_per_launch": conv_us}
         # (3) the short-K transformer linears (HBM / epilogue bound): attention out-projection 320 -> 320 + residual
         T = Bn * 4096
@@ -388,17 +389,15 @@ def main():
 
     if rank != 0:
         return
-    peak_tf, peak_gbs, peak_src = _peaks()
-    burst_tf = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("bf16_tflops", 1736.7) \
-        if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 1590.0
+    peak_tf, peak_gbs = H100_FP16_TFLOPS, H100_HBM_GBS
     k_ach = kern["flop_per_launch"] / (kern["us_per_launch"] * 1e-6) / 1e12
     attn_tf = attn_flop / (attn_us * 1e-6) / 1e12
     # exponential floor of the attention kernel: one ex2 per score at 16 / clk / SM.  The kernel is timed ALONE (it then
     # runs near the maximum SM clock, not at the power-capped clock of the sampler), so the floor is taken at sm_max_mhz —
     # the smallest floor, i.e. xu_frac is a lower bound of how close the kernel is to it
-    sm_hz = (clk["sm_max_mhz"] if clk and clk.get("sm_max_mhz") else 1965) * 1e6
-    xu_floor_us = attn_exps / (16.0 * 148 * sm_hz) * 1e6
-    tr_attn, tr_conv = _traffic("attention_self_64x64_d40", 2 * F), _traffic("conv3x3_64x64_320", 2 * F)
+    sm_hz = (clk["sm_max_mhz"] if clk and clk.get("sm_max_mhz") else 1980) * 1e6
+    n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
+    xu_floor_us = attn_exps / (16.0 * n_sm * sm_hz) * 1e6
     achieved_tf = value * FLOP_PER_FRAME["sd14"] / 1e12 / world
     pro, per_step, vae_l = eng.launches()
     launches_per_call = pro + 1 + n_unet_calls * (per_step + 1) + vae_l
@@ -408,26 +407,26 @@ def main():
         "vs_baseline": None, "dtype": "f16", "data": "synthetic",
         "config": {"workload": workload, "frames_per_step": F, "unet_calls_per_frame": n_unet_calls,
                    "unet_batch": 2 * F, "parallelism": f"frame-dp{world}", "cuda_graph": not a.no_graph,
-                   "l2": "working set per step (1.8 GB weights + activations) exceeds the 126 MB L2"},
+                   "l2": "working set per step (1.8 GB weights + activations) exceeds the 50 MB L2",
+                   "gpu": torch.cuda.get_device_name(dev)},
         "roofline": {
-            "bound": "tensor", "achieved": attn_tf, "peak": burst_tf, "unit": "TFLOP/s", "frac": attn_tf / burst_tf,
-            "traffic": tr_attn["bytes"], "traffic_source": tr_attn["source"],
-            "kernel": "attn_pp_kernel self-attention 64x64, 8 heads x 40 (dominant kernel by share of the step)",
+            "bound": "tensor", "achieved": attn_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": attn_tf / peak_tf,
+            "traffic": None, "traffic_source": "not measured",
+            "kernel": "attn_kernel self-attention 64x64, 8 heads x 40 (dominant kernel by share of the step)",
             "kernel_batch": 2 * F, "us_per_launch": attn_us,
             "xu_floor_us": xu_floor_us, "xu_frac": xu_floor_us / attn_us,
-            "note": f"timed alone, L2 flushed between launches, vs {peak_src} burst fp16/bf16 peak; this kernel is bound by "
-                    "one exponential per score (MUFU.EX2, 16/clk/SM; the kernel moves a quarter of them to the FMA pipe): "
-                    "xu_frac = all-MUFU exponential floor at the maximum SM clock / time",
+            "note": "timed alone, L2 flushed between launches, vs the H100 SXM data-sheet dense fp16 peak; "
+                    "xu_frac = exponential floor (one MUFU.EX2 per score, 16/clk/SM) at the maximum SM clock / time",
             "conv3x3": {"kernel": kern["name"], "kernel_batch": kern["batch"], "us_per_launch": kern["us_per_launch"],
-                        "bound": "tensor", "achieved": k_ach, "peak": burst_tf, "unit": "TFLOP/s", "frac": k_ach / burst_tf,
-                        "traffic": tr_conv["bytes"], "traffic_source": tr_conv["source"]},
-            "short_k_linear": {"kernel": "gemm2_tc_kernel attention out-projection 64x64 320->320 bias+residual",
+                        "bound": "tensor", "achieved": k_ach, "peak": peak_tf, "unit": "TFLOP/s", "frac": k_ach / peak_tf,
+                        "traffic": None, "traffic_source": "not measured"},
+            "short_k_linear": {"kernel": "gemm_kernel attention out-projection 64x64 320->320 bias+residual",
                                "kernel_batch": 2 * F, "us_per_launch": lin_us, "bound": "hbm",
                                "achieved": lin_bytes / (lin_us * 1e-6) / 1e9, "peak": peak_gbs, "unit": "GB/s",
                                "frac": lin_bytes / (lin_us * 1e-6) / 1e9 / peak_gbs,
                                "note": "algorithmic bytes (activations in + residual in + out + weights) / time"},
             "whole_sampler": {"achieved": achieved_tf, "peak": peak_tf, "frac": achieved_tf / peak_tf, "unit": "TFLOP/s",
-                              "note": "frames x 84.45 TFLOP / time / gpus vs sustained peak"}},
+                              "note": "frames x 84.45 TFLOP / time / gpus vs the data-sheet dense fp16 peak"}},
         "e2e": {"value": e2e_val, "unit": "frames/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
         "gpu_launches": launches_per_call * K,
         "clocks": clk,

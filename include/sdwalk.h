@@ -1,4 +1,4 @@
-/* sdwalk.h — C ABI of libsdwalk.so, the Blackwell-native (sm_100a) implementation of the
+/* sdwalk.h — C ABI of libsdwalk.so, the Hopper-native (H100, sm_90a) implementation of the
  * latent-walk hot path of nateraw/stable-diffusion-videos.
  *
  * The reference has no FFI: its hot path sits behind the Python class
@@ -160,7 +160,7 @@ int sdw_engine_debug_vae(sdw_engine* e, const float* latents_nchw, uint8_t* out_
 int sdw_engine_debug_profile(sdw_engine* e, const char* path, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Low-level tensor-core op (tests / tooling): one implicit GEMM on the tcgen05 kernel.
+ * Low-level tensor-core op (tests / tooling): one implicit GEMM on the wgmma kernel.
  * Covers Conv2d 3x3 (stride 1/2, nearest-up x2 fused), 1x1, Linear and batched matmul.
  * ---------------------------------------------------------------------------------------- */
 typedef struct sdw_gemm_desc {
@@ -190,22 +190,21 @@ typedef struct sdw_gemm_desc {
   void* vt;
   int64_t vt_ld;
   int32_t bn;                /* BLOCK_N: 0 auto, 64/128/160/256 */
-  int32_t ver;               /* 0 auto, 1: one CTA per 128xBN tile, 2: persistent CTA pairs (256xBN) */
-  int32_t nsub;              /* 0 auto, 1 / 2: accumulators per activation tile in the CTA-pair kernel */
-  int32_t ew;                /* 0 auto, 2 / 4: epilogue warps per TMEM lane quarter of the CTA-pair kernel (4: needs the TMA epilogue) */
+  int32_t ver;               /* 0 auto, 1: single CTAs, 2: CTA pairs (clusters of two sharing each weight tile by multicast) */
+  int32_t nsub;              /* 0 auto, 1 / 2: accumulators per activation tile (2: CTA pairs, BLOCK_N 160) */
+  int32_t ew;                /* 0 auto or 2: epilogue warps per 32 accumulator rows (the kernel has one epilogue width) */
   int32_t tr;                /* 0 auto, 1 never, 2 require: 3x3 taps reuse one activation box in shared memory */
-  int32_t et;                /* 0 auto, 1 never, 2 require: TMA-store epilogue with a TMA-fed residual ring.  With mode 2 the
-                              * V^T rows are written through TMA, which clips the token extent at 16-byte granularity: the
-                              * vt_ld padding up to the next multiple of 8 tokens may receive finite filler values */
+  int32_t et;                /* 0 auto, 1 never, 2 require: output chunks staged in shared memory and written by TMA stores
+                              * (with mode 2 the V^T rows are still scattered directly) */
   int32_t reserved0;         /* must be 0 */
 } sdw_gemm_desc;
 
 int sdw_gemm(const sdw_gemm_desc* desc, void* stream);
 /* planner introspection, host only (also in plan-only mode): out = {kernel version, BLOCK_N, accumulators, epilogue warps
- * per lane quarter, tap reuse, TMA epilogue, pipeline stages, 0, grid size, tile w, tile h, tile b} */
+ * per 32 rows, tap reuse, TMA epilogue, pipeline stages, 0, grid size, tile w, tile h, tile b} */
 int sdw_debug_plan(const sdw_gemm_desc* desc, int32_t out[12]);
 
-/* fused attention on tcgen05 (tests / tooling): O = softmax(Q K^T d^-1/2) V per (batch, head).
+/* fused attention on wgmma (tests / tooling): O = softmax(Q K^T d^-1/2) V per (batch, head).
  * q [B][Nq][q_ld], k [B][Nk][k_ld] with head h at columns h*d; vt [B][heads][d][vt_ld] = V transposed;
  * out [B][Nq][out_ld]; all fp16; d a multiple of 8 in 8..160. */
 int sdw_attention(const void* q, int64_t q_ld, const void* k, int64_t k_ld, const void* vt, int64_t vt_ld, int B,
@@ -221,9 +220,6 @@ int sdw_layernorm(const void* x, int64_t ldx, int64_t rows, int C, const float* 
 
 /* attention planner introspection, host only: out = {kernel variant, query tiles per CTA, grid x, y, z} */
 int sdw_debug_attention_plan(int B, int Nq, int Nk, int heads, int d, int32_t out[5]);
-/* tooling: device buffer of 2 x 4096 x 8 int64 that CTA 0 of the two-tile attention kernel fills with clock64 stamps per
- * KV tile (wait start, S ready, row in registers, max done, MUFU token held, burst issued, P stored) for query tiles A and B; NULL switches it off */
-void sdw_debug_attention_trace(void* buf);
 
 /* pack an OIHW fp16 conv / [N][K] linear weight into the kernel's K-major [N][taps][Cp] layout */
 int sdw_pack_weight(const void* w_oihw, int N, int C, int kh, int kw, int geglu_interleave, void* out, void* stream);

@@ -1,4 +1,4 @@
-"""stable-diffusion-videos_b200 — Blackwell-native latent-walk hot path.
+"""stable-diffusion-videos_b200 — Hopper-native (H100, sm_90a) latent-walk hot path.
 
 Drop-in surface for the hot path of `stable_diffusion_videos` (reference __init__.py:99-119): import this package
 as `stable_diffusion_videos_b200` and use `StableDiffusionWalkPipeline` / `make_video_pyav` / `get_timesteps_arr`

@@ -50,7 +50,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise SdwError(
                 f"{LIB_PATH} not built: run `python __graft_entry__.py build` "
-                "(the native sm_100a library is required; there is no fallback path)")
+                "(the native sm_90a library is required; there is no fallback path)")
         _lib = C.CDLL(LIB_PATH)
         _lib.sdw_last_error.restype = C.c_char_p
     return _lib
@@ -94,7 +94,7 @@ def slerp_lerp_batch(lat_a, lat_b, emb_a, emb_b, t, dot_threshold=0.9995):
 
 
 def pack_weight(w, geglu=False):
-    """OIHW / [N,K] fp16 weight -> K-major [N][taps][ceil64(C)] layout of the tcgen05 kernel."""
+    """OIHW / [N,K] fp16 weight -> K-major [N][taps][ceil64(C)] layout of the GEMM kernel."""
     require_cuda(w)
     w = w.to(torch.float16).contiguous()
     if w.dim() == 2:

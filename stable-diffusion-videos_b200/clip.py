@@ -23,7 +23,7 @@ class NativeCLIPTextEncoder:
                  num_attention_heads=12, intermediate_size=3072, hidden_act="quick_gelu", layer_norm_eps=1e-5,
                  max_batch=8, device=None):
         if not torch.cuda.is_available():
-            raise N.SdwError("the native CLIP text encoder needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise N.SdwError("the native CLIP text encoder needs a CUDA device (sm_90a); there is no CPU fallback")
         if hidden_act not in ("quick_gelu", "gelu"):
             raise ValueError(f"hidden_act {hidden_act!r}: quick_gelu (SD-1.x) or gelu (SD-2.x) only")
         self.device = torch.device(device or f"cuda:{torch.cuda.current_device()}")

@@ -9,7 +9,7 @@ namespace sdw {
 static thread_local std::string g_err;
 void set_error(const std::string& msg) { g_err = msg; }
 bool pdl_enabled() {
-  static const bool on = [] { const char* e = std::getenv("SDW_PDL"); return e && e[0] == '1'; }();  // measured no gain: opt-in
+  static const bool on = [] { const char* e = std::getenv("SDW_PDL"); return e && e[0] == '1'; }();  // opt-in
   return on;
 }
 const char* last_error() { return g_err.c_str(); }
@@ -120,8 +120,6 @@ int sdw_layernorm(const void* x, int64_t ldx, int64_t rows, int C, const float* 
   return layernorm(static_cast<const __half*>(x), ldx, rows, C, gamma, beta, eps, static_cast<__half*>(y), ldy,
                    static_cast<cudaStream_t>(stream));
 }
-
-void sdw_debug_attention_trace(void* buf) { sdw::attention_set_trace(static_cast<long long*>(buf)); }
 
 int sdw_debug_attention_plan(int B, int Nq, int Nk, int heads, int d, int32_t out[5]) {
   SDW_REQUIRE(out != nullptr, "null");

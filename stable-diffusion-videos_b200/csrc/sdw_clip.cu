@@ -4,7 +4,7 @@
 //
 // SD-1.x: ViT-L/14 text tower (12 layers, 768 wide, 12 heads x 64, MLP 3072, quick-GELU); SD-2.x: OpenCLIP-H (23 used
 // layers, 1024 wide, 16 heads x 64, MLP 4096, GELU) — both are configurations of this engine.  The linears run on the
-// tcgen05 GEMM of sdw_gemm.cu (M = 77 B rows: one or two 128-row tiles), LayerNorm on sdw_norm.cu's kernel; the
+// wgmma GEMM of sdw_gemm.cu (M = 77 B rows: one or two 128-row tiles), LayerNorm on sdw_norm.cu's kernel; the
 // 77 x 77 causal attention per head and the embedding gather are small CUDA-core kernels here (13 GFLOP per prompt: the
 // tower is a feed of the hot loop, not part of it).  State-dict names are transformers' `CLIPTextModel` keys.
 #include "sdw_internal.h"

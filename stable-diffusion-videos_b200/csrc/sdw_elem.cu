@@ -4,7 +4,7 @@
 //   * classifier-free-guidance combine + linear-multistep scheduler update (+ next model input)
 //       reference: stable_diffusion_pipeline.py:414-415, 421-426
 //   * latent state initialisation (latents * init_noise_sigma)  — stable_diffusion_pipeline.py:401
-//   * weight packing into the tcgen05 kernel's K-major layout
+//   * weight packing into the GEMM kernel's K-major layout
 #include "sdw_internal.h"
 #include "sdw_ptx.cuh"
 
@@ -269,7 +269,7 @@ int pack_weight_up4(const void* w, int N, int C, void* out, cudaStream_t stream)
   SDW_REQUIRE(w && out && N > 0 && C > 0, "bad weight");
   const int Cp = (C + 63) / 64 * 64;
   const int64_t total = static_cast<int64_t>(N) * 16 * Cp;
-  const unsigned blocks = static_cast<unsigned>(std::min<int64_t>((total + 255) / 256, 148 * 16));
+  const unsigned blocks = static_cast<unsigned>(std::min<int64_t>((total + 255) / 256, static_cast<int64_t>(sm_count()) * 16));
   pack_weight_up4_kernel<<<blocks, 256, 0, stream>>>(static_cast<const __half*>(w), N, C, Cp, static_cast<__half*>(out));
   SDW_CUDA_OK(cudaGetLastError());
   return 0;
@@ -281,7 +281,7 @@ int pack_weight(const void* w, int N, int C, int kh, int kw, int geglu, void* ou
   const int Cp = (C + 63) / 64 * 64;
   const int64_t total = static_cast<int64_t>(N) * kh * kw * Cp;
   const int threads = 256;
-  const unsigned blocks = static_cast<unsigned>(std::min<int64_t>((total + threads - 1) / threads, 148 * 16));
+  const unsigned blocks = static_cast<unsigned>(std::min<int64_t>((total + threads - 1) / threads, static_cast<int64_t>(sm_count()) * 16));
   pack_weight_kernel<<<blocks, threads, 0, stream>>>(static_cast<const __half*>(w), N, C, kh * kw, Cp, geglu,
                                                      static_cast<__half*>(out));
   SDW_CUDA_OK(cudaGetLastError());

@@ -221,7 +221,7 @@ struct Engine {
   }
   // tiled = True: circular padding (reference P:841-858 patches every Conv2d to padding_mode="circular").  A 3x3 conv on the
   // torus = the zero-padded conv of the wrap-padded image, cropped: pad (1 pixel; 2 for the stride-2 conv so that the
-  // output centres stay on even coordinates), run the unchanged tcgen05 kernel on the padded lattice, crop (+ residual).
+  // output centres stay on even coordinates), run the unchanged GEMM kernel on the padded lattice, crop (+ residual).
   bool tiled = false;
   int conv(const T& x, const __half* w, const float* bias, int N, int kind, const T& out, const T* resid = nullptr,
            const float* rowvec_table = nullptr, int mode = GEMM_PLAIN) {
@@ -327,7 +327,7 @@ struct Engine {
   int cfg_groups = 32;
   bool use_flash = true;
 
-  // unfused attention: S = alpha Q K^T (head-batched tcgen05 GEMM) ; softmax rows ; O = P V
+  // unfused attention: S = alpha Q K^T (head-batched GEMM) ; softmax rows ; O = P V
   int attention(const __half* q, int64_t q_ld, const __half* k, int64_t k_ld, const __half* vt, int64_t vt_ld, int Bq,
                 int Nq, int Nk, int heads, int d, const T& out) {
     if (use_flash && attn_supported(d)) {
@@ -817,7 +817,7 @@ __global__ void ctx_assemble_kernel(const __half* __restrict__ cond, const __hal
 }
 int unet_ctx_assemble(const __half* cond, const __half* uncond, int F, int dup, int64_t per, __half* out,
                       cudaStream_t stream, int uncond_per_frame = 0) {
-  ctx_assemble_kernel<<<148 * 2, 256, 0, stream>>>(cond, uncond, F, dup, per, out, uncond_per_frame);
+  ctx_assemble_kernel<<<sm_count() * 2, 256, 0, stream>>>(cond, uncond, F, dup, per, out, uncond_per_frame);
   SDW_CUDA_OK(cudaGetLastError());
   return 0;
 }

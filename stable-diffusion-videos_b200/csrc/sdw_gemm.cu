@@ -1,19 +1,26 @@
-// sdw_gemm.cu — the tcgen05 implicit-GEMM kernel behind every Conv2d 3x3 / 1x1,
-// Linear and batched matmul of the UNet2DCondition / AutoencoderKL-decoder hot path
-// (reference call sites: stable_diffusion_pipeline.py:418 `self.unet(...)`, :433 `self.vae.decode`).
+// sdw_gemm.cu — the wgmma implicit-GEMM kernel behind every Conv2d 3x3 / 1x1, Linear and batched matmul of the
+// UNet2DCondition / AutoencoderKL-decoder hot path (reference call sites: stable_diffusion_pipeline.py:418
+// `self.unet(...)`, :433 `self.vae.decode`).
 //
-// Shape of the kernel (one 128 x BN output tile per CTA, 2 CTAs co-resident per SM):
-//   warp 0    : TMA producer — per K block (tap, 64-channel chunk) one 4-D box load of the
-//               shifted NHWC activation tile (OOB halo = zero fill = conv padding) and one
-//               box of the K-major weight tile, SWIZZLE_128B, into a STAGES-deep smem ring.
-//   warp 1    : TMEM allocator + MMA issuer — one elected thread issues 4 x tcgen05.mma
-//               (M=128, N=BN, K=16) per K block, accumulating fp32 in TMEM; tcgen05.commit
-//               releases the smem stage / signals the epilogue.
-//   warps 2-5 : epilogue — tcgen05.ld the accumulator (thread = output row), fuse
-//               alpha / bias / time-embedding row vector / SiLU / residual / GEGLU /
-//               per-head V^T scatter, write fp16.
+// One CTA computes 128 x (NSUB * BN) output tiles, persistent over a static round-robin of tiles (N fastest, so the
+// column tiles of one activation tile run at the same time and the activation tile leaves DRAM once):
+//   warps 0-7 : two consumer warpgroups, rows 0-63 / 64-127 of the tile.  Per K block (tap, 64-channel chunk) each
+//               issues 4 x wgmma m64nBNk16 per accumulator from the shared-memory ring (fp32 accumulators in registers,
+//               one wgmma group kept in flight), then runs the fused epilogue of the tile from its registers:
+//               alpha / bias / time-embedding row vector / SiLU / residual / GEGLU / per-head V^T scatter, fp16 out,
+//               either stored directly or staged per 32-column chunk in shared memory and written by TMA stores.
+//   warp 8    : TMA producer — per K block one 4-D box of the shifted NHWC activation tile (OOB halo = zero fill =
+//               conv padding) and the K-major weight tile(s), SWIZZLE_128B, into an nstages-deep ring.
+//
+// CL = 2 (the CTA-pair plan): two CTAs of a cluster work on vertically adjacent M tiles with the same weight tile.
+// Each loads its own activation rows and HALF of the weight tile, multicast into both CTAs' shared memory, so weight
+// bytes per tile fetched from L2 halve; a stage is released only when the consumers of both CTAs are done with it.
+//
+// TR = 1 (tap reuse, 3x3 stride-1 convs on 16 x 8-pixel tiles): the three ky taps of one kx read the same pixels
+// shifted by whole image rows, so one TMA box of (8 + 2) rows x 16 px x 64 ch per (channel chunk, kx) serves three
+// taps: tap ky's A operand is the same shared-memory tile entered 16 rows (2 KB, swizzle-atom aligned) further down.
+// NSUB = 2: two accumulators per activation tile (128 x 2*BN tiles).
 #include "sdw_internal.h"
-#include "sdw_gemm_epi.cuh"
 #include "sdw_ptx.cuh"
 
 #include <cudaTypedefs.h>
@@ -26,120 +33,385 @@ namespace sdw {
 
 static constexpr int BM = 128;
 static constexpr int BK = 64;
-static constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KiB
-static constexpr int GEMM_THREADS = 192;
+static constexpr int GEMM_THREADS = 288;  // two consumer warpgroups + one producer warp
+static constexpr int A_STAGE = BM * BK * 2;  // 16 KiB
+static constexpr int TR_BW = 16, TR_BH = 8;
+static constexpr int A_STAGE_TR = (TR_BH + 2) * TR_BW * 128;  // 20 KiB
 
-template <int BN>
+template <int BN, int NSUB, int TR>
 struct GemmCfg {
-  static constexpr int B_STAGE_BYTES = BN * BK * 2;
-  static constexpr int STAGES = (BN <= 64) ? 4 : (BN <= 160 ? 3 : 4);
-  static constexpr int TMEM_COLS = BN <= 32 ? 32 : (BN <= 64 ? 64 : (BN <= 128 ? 128 : 256));
-  static constexpr int SMEM_BYTES = STAGES * (A_STAGE_BYTES + B_STAGE_BYTES) + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int A_BYTES = TR ? A_STAGE_TR : A_STAGE;
+  static constexpr int TAPS = TR ? 3 : 1;  // weight tiles (taps) per pipeline stage
+  static constexpr int B_SUB = BN * 128;   // one BN-row weight tile
+  static constexpr int B_BYTES = TAPS * NSUB * B_SUB;
 };
 
+struct EpiRow {
+  bool ok;
+  int64_t out_off, res_off, pix;
+  const float* rowvec;
+};
+
+// fused epilogue of one accumulator (columns n_base .. n_base + BN) of this warpgroup's 64 rows
 template <int BN>
-__global__ void __launch_bounds__(GEMM_THREADS) gemm_tc_kernel(const __grid_constant__ GemmKParams p) {
-  using Cfg = GemmCfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
+__device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)[BN / 2], int n_base, const EpiRow (&R)[2],
+                                              int lane, int wg, int lrow0, uint8_t* stage, uint64_t* res_full, int x0,
+                                              int y0, int b0, uint32_t& chunk_count) {
+  const int q2 = 2 * (lane & 3);
+  const bool vec2 = p.vec2;
+  const bool use_tma = p.epi_tma;
+  // TMA origin of this warpgroup's 64 rows: a (hw, hh, hb) sub-box of the (bw, bh, bb) tile
+  const int r0 = 64 * wg;
+  const int tx = x0 + (r0 & (p.bw - 1)), ty = y0 + ((r0 >> p.lg_bw) & (p.bh - 1)), tb = b0 + (r0 >> (p.lg_bw + p.lg_bh));
+  const bool issuer = (threadIdx.x & 127) == 0;
+  // TMA epilogue with a residual: chunk k's [64 rows x 32 columns] residual arrives by TMA in output buffer k & 1 itself
+  // (each thread overwrites exactly the elements it reads), issued one chunk ahead — the first one before this
+  // accumulator's first chunk — once the TMA store that last used the buffer has read it
+  const bool tma_res = use_tma && p.resid != nullptr;
+  const int nch = (min(BN, p.N - n_base) + 31) >> 5;
+  auto res_issue = [&](int c, uint32_t k) {
+    if (tma_res && issuer && c < nch) {
+      mbar_expect_tx(&res_full[k & 1], 4096);
+      tma_load_4d(&p.mapRes, &res_full[k & 1], stage + (k & 1) * 4096, n_base + 32 * c, tx, ty, tb);
+    }
+  };
+  if (tma_res && p.mode == GEMM_PLAIN) {
+    if (issuer) bulk_wait_group_read<1>();
+    res_issue(0, chunk_count);
+  }
+
+  auto value = [&](float v, int n, int h) {
+    float o = v * p.alpha;
+    if (p.bias) o += __ldg(p.bias + n);
+    if (p.rowvec) o += __ldg(R[h].rowvec + n);
+    if (p.act == 1) o = silu_f(o);
+    return o;
+  };
+  // 2 x 2 values (rows h = 0 / 1, columns n, n + 1) of the plain path, residual added, stored or staged
+  auto plain_pair = [&](int j, int n, uint8_t* staged, int scol) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float o0 = n < p.N ? value(acc[4 * j + 2 * h], n, h) : 0.f;
+      float o1 = n + 1 < p.N ? value(acc[4 * j + 2 * h + 1], n + 1, h) : 0.f;
+      if (staged && tma_res) {
+        const float2 f =
+            __half22float2(*reinterpret_cast<const __half2*>(staged + (lrow0 + 8 * h) * 64 + scol * 2));
+        o0 += f.x;
+        o1 += f.y;
+      } else if (p.resid && R[h].ok) {
+        if (vec2 && n + 1 < p.N) {
+          const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.resid + R[h].res_off + n));
+          o0 += f.x;
+          o1 += f.y;
+        } else {
+          if (n < p.N) o0 += __half2float(p.resid[R[h].res_off + n]);
+          if (n + 1 < p.N) o1 += __half2float(p.resid[R[h].res_off + n + 1]);
+        }
+      }
+      if (staged) {
+        *reinterpret_cast<uint32_t*>(staged + (lrow0 + 8 * h) * 64 + scol * 2) = pack_h2(o0, o1);
+      } else if (R[h].ok) {
+        __half* dst = p.out + R[h].out_off + n;
+        if (vec2 && n + 1 < p.N) {
+          *reinterpret_cast<uint32_t*>(dst) = pack_h2(o0, o1);
+        } else {
+          if (n < p.N) dst[0] = __float2half_rn(o0);
+          if (n + 1 < p.N) dst[1] = __float2half_rn(o1);
+        }
+      }
+    }
+  };
+  // V^T scatter (columns >= vt_col0): element (b, head, dd, token)
+  auto vt_pair = [&](int j, int n) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!R[h].ok) continue;
+      const int64_t bq = R[h].pix / p.vt_ntok;
+      const int tok = static_cast<int>(R[h].pix - bq * p.vt_ntok);
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int nn = n + e;
+        if (nn >= p.N) continue;
+        float o = acc[4 * j + 2 * h + e] * p.alpha;
+        if (p.bias) o += __ldg(p.bias + nn);
+        const int cc = nn - p.vt_col0, head = cc / p.vt_d, dd = cc - head * p.vt_d;
+        p.vt[((bq * p.vt_heads + head) * p.vt_d + dd) * p.vt_ld + tok] = __float2half_rn(o);
+      }
+    }
+  };
+  // staged chunk (two 4 KB buffers per warpgroup, alternating): wait until the TMA store that last read the buffer is
+  // done, fill it, hand it to the async proxy, store
+  auto stage_begin = [&]() {
+    if (issuer) bulk_wait_group_read<1>();
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+    return stage + (chunk_count & 1) * 4096;
+  };
+  auto stage_end = [&](uint8_t* buf, int col) {
+    fence_proxy_async_smem();
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+    if (issuer) {
+      tma_store_4d(&p.mapOut, buf, col, tx, ty, tb);
+      bulk_commit_group();
+    }
+    ++chunk_count;
+  };
+
+  if (p.mode == GEMM_GEGLU) {
+    // packed [32 value | 32 gate] column pairs -> 32 outputs a * gelu(g) per 64 accumulator columns
+#pragma unroll
+    for (int c = 0; c < BN / 64; ++c) {
+      const int n = n_base + 64 * c;
+      if (n >= p.N) break;
+      uint8_t* buf = use_tma ? stage_begin() : nullptr;
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 8 * c + jj;
+        const int na = n + 8 * jj + q2, ng = na + 32;
+        float o[2][2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float a = acc[4 * j + 2 * h + e] * p.alpha, g = acc[4 * (j + 4) + 2 * h + e] * p.alpha;
+            if (p.bias) {
+              a += __ldg(p.bias + na + e);
+              g += __ldg(p.bias + ng + e);
+            }
+            o[h][e] = geglu_f(a, g);
+          }
+        const int ocol = n / 2 + 8 * jj + q2;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (use_tma) {
+            *reinterpret_cast<uint32_t*>(buf + (lrow0 + 8 * h) * 64 + (8 * jj + q2) * 2) = pack_h2(o[h][0], o[h][1]);
+          } else if (R[h].ok) {
+            __half* dst = p.out + R[h].out_off + ocol;
+            if (vec2) {
+              *reinterpret_cast<uint32_t*>(dst) = pack_h2(o[h][0], o[h][1]);
+            } else {
+              dst[0] = __float2half_rn(o[h][0]);
+              dst[1] = __float2half_rn(o[h][1]);
+            }
+          }
+        }
+      }
+      if (use_tma) stage_end(buf, n / 2);
+    }
+    return;
+  }
+#pragma unroll
+  for (int c = 0; c < BN / 32; ++c) {
+    const int n = n_base + 32 * c;
+    if (n >= p.N) break;
+    if (p.mode == GEMM_QKV_VT && n >= p.vt_col0) {  // vt_col0 % 32 == 0: a chunk is all Q|K or all V
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) vt_pair(4 * c + jj, n + 8 * jj + q2);
+      continue;
+    }
+    if (use_tma) {
+      uint8_t* buf = stage_begin();
+      if (tma_res) {
+        if (issuer && c + 1 < nch) bulk_wait_group_read<0>();  // the previous chunk's store has read the other buffer
+        res_issue(c + 1, chunk_count + 1);
+        mbar_wait(&res_full[chunk_count & 1], (chunk_count >> 1) & 1);
+      }
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) plain_pair(4 * c + jj, n + 8 * jj + q2, buf, 8 * jj + q2);
+      stage_end(buf, n);
+    } else {
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) plain_pair(4 * c + jj, n + 8 * jj + q2, nullptr, 0);
+    }
+  }
+}
+
+template <int BN, int NSUB, int TR, int CL>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_constant__ GemmKParams p) {
+  using Cfg = GemmCfg<BN, NSUB, TR>;
+  constexpr int A_BYTES = Cfg::A_BYTES;
+  constexpr int B_BYTES = Cfg::B_BYTES;
+  const int STAGES = p.nstages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * A_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + STAGES * Cfg::B_STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem);
+  uint64_t* empty_bar = full_bar + GEMM_MAX_STAGES;
+  uint8_t* smem_a = smem + GEMM_BAR_BYTES;
+  uint8_t* smem_b = smem_a + STAGES * A_BYTES;
+  uint8_t* epi_stage = smem_b + STAGES * B_BYTES;  // epi_tma: 2 x 4 KB output buffers per consumer warpgroup
+  uint64_t* res_full = empty_bar + GEMM_MAX_STAGES;  // [2 warpgroups][2 buffers]: residual chunk arrived
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t rank = CL > 1 ? cluster_ctarank() : 0;
+  const int cluster_id = blockIdx.x / CL;
+  const int nclusters = gridDim.x / CL;
+  const int total_tiles = p.m_groups * p.n_tiles;
+  const int num_kb = TR ? 3 * p.kchunks : p.ntaps * p.kchunks;
 
-  // ---- tile coordinates -------------------------------------------------
-  const int m_tile = blockIdx.x;
-  const int tw = m_tile % p.tiles_w;
-  const int th = (m_tile / p.tiles_w) % p.tiles_h;
-  const int tb = m_tile / (p.tiles_w * p.tiles_h);
-  const int x0 = tw * p.bw, y0 = th * p.bh, b0 = tb * p.bb;
-  const int n0 = blockIdx.y * BN;
-  const int num_kb = p.ntaps * p.kchunks;
-
-  // ---- one-time setup -----------------------------------------------------
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&p.mapA[0]);
     tma_prefetch_desc(&p.mapB);
+    if (p.epi_tma) tma_prefetch_desc(&p.mapOut);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 2 * CL);  // both consumer warpgroups of every CTA that reads the stage's weight halves
     }
-    mbar_init(tmem_full_bar, 1);
+    for (int i = 0; i < 4; ++i) mbar_init(&res_full[i], 1);
+    if (p.epi_tma && p.resid) tma_prefetch_desc(&p.mapRes);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_ptr_smem, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = *tmem_ptr_smem;
-  pdl_wait();
+  if (CL > 1) cluster_sync_all();
+  else __syncthreads();
+  pdl_wait();               // the set-up above overlapped the previous kernel's tail; its outputs are visible from here
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  auto tile_coords = [&](int t, int& x0, int& y0, int& b0, int& n0) {
+    const int m_group = t / p.n_tiles;
+    const int n_tile = t - m_group * p.n_tiles;
+    const int m_tile = m_group * CL + static_cast<int>(rank);
+    const int twh = p.tiles_w * p.tiles_h;
+    const int tb = m_tile / twh;
+    const int rem = m_tile - tb * twh;
+    const int th = rem / p.tiles_w;
+    const int tw = rem - th * p.tiles_w;
+    x0 = tw * p.bw;
+    y0 = th * p.bh;
+    b0 = tb * p.bb;
+    n0 = n_tile * (NSUB * BN);
+  };
+
+  if (warp == 8) {
     // =========================== TMA producer ===============================
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        const int tap = kb / p.kchunks;
-        const int kc = kb - tap * p.kchunks;
-        mbar_expect_tx(&full_bar[stage], A_STAGE_BYTES + Cfg::B_STAGE_BYTES);
-        tma_load_4d(&p.mapA[p.tap_map[tap]], &full_bar[stage], smem_a + stage * A_STAGE_BYTES, kc * BK,
-                    x0 + p.tap_dx[tap], y0 + p.tap_dy[tap], b0);
-        tma_load_4d(&p.mapB, &full_bar[stage], smem_b + stage * Cfg::B_STAGE_BYTES, kb * BK, n0,
-                    p.b_batched ? y0 : 0, p.b_batched ? b0 : 0);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===================================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_f16(BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint64_t da = make_desc_k_sw128(smem_u32(smem_a + stage * A_STAGE_BYTES));
-        const uint64_t db = make_desc_k_sw128(smem_u32(smem_b + stage * Cfg::B_STAGE_BYTES));
+      for (int t = cluster_id; t < total_tiles; t += nclusters) {
+        int x0, y0, b0, n0;
+        tile_coords(t, x0, y0, b0, n0);
+        int tap = 0, kc = 0;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          mbar_expect_tx(&full_bar[stage], A_BYTES + B_BYTES);  // with CL = 2 half of B arrives from the peer CTA
+          uint8_t* a_dst = smem_a + stage * A_BYTES;
+          uint8_t* b_dst = smem_b + stage * B_BYTES + rank * (BN / CL) * 128;
+          const int nrow = n0 + static_cast<int>(rank) * (BN / CL);
+          if (TR) {
+            const int kx = tap;  // tap reuse: `tap` counts the column tap kx = 0..2 of channel chunk kc
+            tma_load_4d(&p.mapA[0], &full_bar[stage], a_dst, kc * BK, x0 + kx - 1, y0 - 1, b0);
+          } else {
+            tma_load_4d(&p.mapA[p.tap_map[tap]], &full_bar[stage], a_dst, kc * BK, x0 + p.tap_dx[tap], y0 + p.tap_dy[tap],
+                        b0);
+          }
 #pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          // advance 16 fp16 = 32 B inside the 128-B swizzle row: +2 in the (>>4) address field
-          umma_f16_ss(tmem_acc, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[stage]);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
+          for (int ky = 0; ky < Cfg::TAPS; ++ky)
+#pragma unroll
+            for (int sub = 0; sub < NSUB; ++sub) {
+              const int kcoord = TR ? ((ky * 3 + tap) * p.kchunks + kc) * BK : kb * BK;
+              uint8_t* dst = b_dst + (ky * NSUB + sub) * Cfg::B_SUB;
+              const int c2 = p.b_batched ? y0 : 0, c3 = p.b_batched ? b0 : 0;
+              if (CL > 1)
+                tma_load_4d_mc(&p.mapB, &full_bar[stage], dst, kcoord, nrow + sub * BN, c2, c3, (1u << CL) - 1);
+              else
+                tma_load_4d(&p.mapB, &full_bar[stage], dst, kcoord, nrow + sub * BN, c2, c3);
+            }
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+          if (TR) {
+            if (++tap == 3) {
+              tap = 0;
+              ++kc;
+            }
+          } else if (++kc == p.kchunks) {
+            kc = 0;
+            ++tap;
+          }
         }
       }
-      umma_commit(tmem_full_bar);
     }
   } else {
-    // =========================== epilogue ======================================
-    gemm_epilogue<BN>(p, tmem_acc, warp, lane, x0, y0, b0, n0, tmem_full_bar);
+    // =========================== consumers: MMA + epilogue ============================
+    const int wg = warp >> 2;
+    const int lrow0 = 16 * (warp & 3) + (lane >> 2);  // this thread's first row within the warpgroup's 64
+    uint8_t* stage_buf = epi_stage + wg * 8192;
+    uint32_t chunk_count = 0;
+    // arrival on the empty barrier of `s` in every CTA of the cluster (one thread per warpgroup)
+    auto release = [&](int s) {
+      if ((threadIdx.x & 127) == 0) {
+        if (CL > 1) {
+#pragma unroll
+          for (int r = 0; r < CL; ++r) mbar_arrive_cluster(mapa_rank(smem_u32(&empty_bar[s]), r));
+        } else {
+          mbar_arrive(&empty_bar[s]);
+        }
+      }
+    };
+    int stage = 0;
+    uint32_t phase = 0;
+    float acc[NSUB][BN / 2];
+    for (int t = cluster_id; t < total_tiles; t += nclusters) {
+      int x0, y0, b0, n0;
+      tile_coords(t, x0, y0, b0, n0);
+#pragma unroll
+      for (int sub = 0; sub < NSUB; ++sub)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[sub][i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_base = smem_u32(smem_a + stage * A_BYTES);
+        const uint32_t b_base = smem_u32(smem_b + stage * B_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int ky = 0; ky < Cfg::TAPS; ++ky) {
+          // rows of this warpgroup: 64 lattice points = 4 image rows of the 16-px tap-reuse tile, entered ky rows down
+          const uint32_t a_off = TR ? (4 * wg + ky) * (TR_BW * 128) : wg * (64 * 128);
+          const uint64_t da = make_desc_k_sw128(a_base + a_off);
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k)
+#pragma unroll
+            for (int sub = 0; sub < NSUB; ++sub) {
+              const uint64_t db = make_desc_k_sw128(b_base + (ky * NSUB + sub) * Cfg::B_SUB);
+              Wgmma<BN>::ss(acc[sub], da + 2 * k, db + 2 * k, (kb | ky | k) != 0 ? 1u : 0u);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous K block's MMAs have read their stage
+        if (prev >= 0) release(prev);
+        prev = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int sub = 0; sub < NSUB; ++sub) reg_fence(acc[sub]);
+      release(prev);
+
+      // ---- epilogue: rows lrow0 and lrow0 + 8 of this warpgroup ----
+      EpiRow R[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = 64 * wg + lrow0 + 8 * h;
+        const int x = x0 + (r & (p.bw - 1)), y = y0 + ((r >> p.lg_bw) & (p.bh - 1)), b = b0 + (r >> (p.lg_bw + p.lg_bh));
+        R[h].ok = x < p.W && y < p.H && b < p.B;
+        R[h].pix = (static_cast<int64_t>(b) * p.H + y) * p.W + x;
+        const int64_t oyy = static_cast<int64_t>(y) * p.os + p.oy, oxx = static_cast<int64_t>(x) * p.os + p.ox;
+        R[h].out_off = static_cast<int64_t>(b) * p.o_sB + oyy * p.o_sH + oxx * p.o_sW;
+        R[h].res_off = static_cast<int64_t>(b) * p.r_sB + oyy * p.r_sH + oxx * p.r_sW;
+        R[h].rowvec = p.rowvec ? p.rowvec + static_cast<int64_t>(b) * p.rowvec_ld : nullptr;
+      }
+#pragma unroll
+      for (int sub = 0; sub < NSUB; ++sub)
+        gemm_epilogue<BN>(p, acc[sub], n0 + sub * BN, R, lane, wg, lrow0, stage_buf, res_full + 2 * wg, x0, y0, b0,
+                          chunk_count);
+    }
+    if (p.epi_tma && (threadIdx.x & 127) == 0) bulk_wait_group<0>();  // every output chunk has reached global memory
   }
 
-  // ---- teardown -------------------------------------------------------------
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_acc, Cfg::TMEM_COLS);
-  }
+  // no CTA of a pair may exit while its peer can still multicast into its shared memory or arrive on its barriers
+  if (CL > 1) cluster_sync_all();
 }
 
 // =============================================================================
@@ -149,11 +421,18 @@ static PFN_cuTensorMapEncodeTiled_v12000 g_encode = nullptr;
 static bool g_plan_only = false;  // validate plans without a driver (CPU-side tests); nothing can be launched
 void set_plan_only(bool on) { g_plan_only = on; }
 
-template <int BN>
-static int set_attr() {
-  SDW_CUDA_OK(cudaFuncSetAttribute(gemm_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   GemmCfg<BN>::SMEM_BYTES));
-  return 0;
+int sm_count() {
+  static int n = 0;
+  if (g_plan_only) return H100_SMS;
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        n <= 0) {
+      (void)cudaGetLastError();
+      n = H100_SMS;
+    }
+  }
+  return n;
 }
 
 int gemm_init() {
@@ -166,14 +445,10 @@ int gemm_init() {
     return 2;
   }
   g_encode = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(fn);
-  if (int e = set_attr<64>()) return e;
-  if (int e = set_attr<128>()) return e;
-  if (int e = set_attr<160>()) return e;
-  if (int e = set_attr<256>()) return e;
   return 0;
 }
 
-// rank-`rank` fp16 tensor map, dim 0 contiguous, SWIZZLE_128B, zero OOB fill.
+// rank-`rank` fp16 tensor map, dim 0 contiguous, zero OOB fill.
 int encode_map(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
                const uint32_t* box, int swizzle_bytes) {
   if (int e = gemm_init()) return e;
@@ -220,6 +495,12 @@ static int pow2_floor(int v) {
   int p = 1;
   while (p * 2 <= v) p *= 2;
   return p;
+}
+
+static int stages_for(int bn, int nsub, bool reuse, int epi_bytes) {
+  const int a = reuse ? A_STAGE_TR : A_STAGE;
+  const int b = (reuse ? 3 : 1) * nsub * bn * 128;
+  return std::min(GEMM_MAX_STAGES, (GEMM_SMEM_USABLE - GEMM_BAR_BYTES - epi_bytes) / (a + b));
 }
 
 int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
@@ -297,108 +578,114 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
   const int tiles_b = (d.B + bb - 1) / bb;
   p.N = d.N;
   p.b_batched = d.b_batched;
-  // kernel version: CTA pairs need >= 2 M tiles and a wide-enough N; batched matmuls must pair within one (h, b)
+  // kernel version: CTA pairs (weight tile multicast to two M tiles) need >= 2 M tiles and a wide-enough N; batched
+  // matmuls must pair within one (h, b)
   const int m_tiles = p.tiles_w * p.tiles_h * tiles_b;
   int ver = d.ver;
-  if (ver == 0) {
-    static const bool force_v1 = [] { const char* e = std::getenv("SDW_GEMM_V1"); return e && e[0] == '1'; }();
-    ver = (!force_v1 && m_tiles >= 2 && d.N >= 128 && (!d.b_batched || p.tiles_w % 2 == 0)) ? 2 : 1;
-  }
-  if (ver == 2) SDW_REQUIRE(!d.b_batched || p.tiles_w % 2 == 0, "2-CTA batched matmul needs an even tile count per row");
+  if (ver == 0) ver = (m_tiles >= 2 && d.N >= 128 && (!d.b_batched || p.tiles_w % 2 == 0)) ? 2 : 1;
+  SDW_REQUIRE(ver == 1 || ver == 2, "unknown kernel version");
+  if (ver == 2) SDW_REQUIRE(!d.b_batched || p.tiles_w % 2 == 0, "CTA-pair batched matmul needs an even tile count per row");
   // tap reuse (3x3 stride 1, CTA pairs): 16 x 8-pixel tiles, one 10-row activation box per (channel chunk, kx)
   bool reuse = false;
   {
-    static const int tr_env = [] { const char* e = std::getenv("SDW_GEMM_TR"); return e ? std::atoi(e) : -1; }();
     const bool can = ver == 2 && d.conv == 1 && Wd % 16 == 0 && Hd % 8 == 0;
     if (d.tr == 2) SDW_REQUIRE(can, "tap reuse needs a 3x3 stride-1 conv on the CTA-pair kernel with W % 16 == 0, H % 8 == 0");
-    reuse = can && d.tr != 1 && (d.tr == 2 || tr_env != 0);
+    reuse = can && d.tr != 1;
     if (reuse) {
-      p.bw = bw = 16;
-      p.bh = bh = 8;
+      p.bw = bw = TR_BW;
+      p.bh = bh = TR_BH;
       p.bb = bb = 1;
-      p.tiles_w = Wd / 16;
-      p.tiles_h = Hd / 8;
+      p.tiles_w = Wd / TR_BW;
+      p.tiles_h = Hd / TR_BH;
     }
   }
-  p.tap_reuse = reuse ? 1 : 0;
-  L->tr = p.tap_reuse;
-  const int m_tiles_f = p.tiles_w * p.tiles_h * ((d.B + bb - 1) / bb);
-  // BLOCK_N choice
+  L->tr = reuse ? 1 : 0;
+  const int CL = ver == 2 ? 2 : 1;
+  const int nsm = sm_count();
+  // ---- epilogue flavour: output chunks staged in shared memory and written by TMA stores where the views allow ----
+  const int ncols = d.mode == GEMM_GEGLU ? d.N / 2 : (d.mode == GEMM_QKV_VT ? d.vt_col0 : d.N);
+  const int64_t osW = d.o_sW || d.o_sH || d.o_sB ? d.o_sW : d.ldc;
+  const int64_t osH = d.o_sW || d.o_sH || d.o_sB ? d.o_sH : OW * d.ldc;
+  const int64_t osB = d.o_sW || d.o_sH || d.o_sB ? d.o_sB : OH * OW * d.ldc;
+  bool can_tma;
+  int64_t res_sW, res_sH, res_sB;
+  {
+    auto ok16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+    auto ok_strides = [&](int64_t sw, int64_t sh, int64_t sb) {
+      return sw > 0 && sw % 8 == 0 && (Hd == 1 || sh % 8 == 0) && (d.B == 1 || sb % 8 == 0);
+    };
+    const bool vt_ok = d.mode != GEMM_QKV_VT || (d.vt_col0 % 32 == 0 && !d.resid);
+    const int64_t ldr = d.ldr ? d.ldr : d.ldc;
+    const bool rs = d.r_sW || d.r_sH || d.r_sB;
+    res_sW = rs ? d.r_sW : ldr;
+    res_sH = rs ? d.r_sH : OW * ldr;
+    res_sB = rs ? d.r_sB : OH * OW * ldr;
+    const bool res_ok = !d.resid || (d.mode == GEMM_PLAIN && ok16(d.resid) && ok_strides(res_sW, res_sH, res_sB));
+    can_tma = !d.b_batched && vt_ok && res_ok && (!d.rowvec || d.rowvec_ld == 0) && d.N % 8 == 0 && ncols > 0 &&
+              ok16(d.out) && ok_strides(osW, osH, osB) && (!d.bias || ok16(d.bias));
+    if (d.et == 2) SDW_REQUIRE(can_tma, "the TMA epilogue needs no per-sample row vector and 16-byte aligned views");
+    p.epi_tma = can_tma && d.et != 1 ? 1 : 0;
+  }
+  const int epi_bytes = p.epi_tma ? GEMM_EPI_BYTES : 0;
+  // ---- BLOCK_N: wgmma runs 2 x 64 x BN x 16 per instruction at a fixed rate, so a tile's mainloop time grows with its
+  // width; the choice minimises waves x tile width (the padded columns of the last N tile included), prefers the wider
+  // tile on a tie (fewer activation reloads) and avoids plans that leave fewer than three pipeline stages ----
   int bn = d.bn;
-  int nsub = 1;
-  if (ver == 2 && (bn == 0 || d.nsub == 2)) {
-    // The 2-CTA kernel is L2->SM bandwidth bound (profiles/r01_mma_eff_vs_blockN.txt): a tile costs about
-    // (16 KB of A + 64 B x columns of W) per K block, so the choice minimises waves x bytes over
-    // BLOCK_N in {256, 192, 160, 128} and, for long-K problems, the two-accumulator 2 x 160 tile (single-buffered TMEM).
-    struct Cand { int bn, nsub; };
-    const Cand cand[5] = {{160, 2}, {256, 1}, {192, 1}, {160, 1}, {128, 1}};
-    const int mp = (m_tiles_f + 1) / 2;
-    const int kblocks = p.ntaps * kchunks;
-    // activation bytes per CTA per K block: a 128 x 64 tile, or a third of the 10-row box; the MMA floor is 2 clk per
-    // column at ~41 B/clk/SM of operand ingest -> 82 "bytes" per column
-    const double a_bytes = reuse ? 20480.0 / 3.0 : 16384.0;
-    double best_cost = 1e30;
-    int best_bn = 128;
-    for (const Cand& c : cand) {
-      if (d.bn && d.bn != c.bn) continue;
-      if (d.nsub && d.nsub != c.nsub) continue;
-      if (d.mode == GEMM_GEGLU && c.bn % 64 != 0) continue;
-      if (c.nsub == 2 && (kblocks < 18 || d.mode != GEMM_PLAIN || reuse) && d.nsub != 2) continue;  // reuse: only 2 stages fit
-      const int width = c.bn * c.nsub;
-      const int tiles = mp * ((d.N + width - 1) / width);
-      const int waves = (tiles + 73) / 74;
-      double cost = static_cast<double>(waves) * std::max(a_bytes + 64.0 * width, 82.0 * width);
-      // measured (profiles/r01_gemm_shapes_tap_reuse.txt): with 3-tap stages only 3 stages of BLOCK_N = 256 fit and the
-      // variant gains nothing over per-tap loads
-      if (reuse && c.bn == 256) cost = static_cast<double>(waves) * 31000.0;
-      if (c.nsub == 2) cost *= 1.0 + 24.0 / kblocks;  // un-overlapped epilogue ~ 24 K-block times (fit: profiles/r01_gemm_shapes_nsub2.txt)
-      if (cost < best_cost) {
-        best_cost = cost;
-        best_bn = c.bn;
-        nsub = c.nsub;
+  int nsub = d.nsub ? d.nsub : 1;
+  SDW_REQUIRE(nsub == 1 || nsub == 2, "one or two accumulators per activation tile");
+  if (nsub == 2) SDW_REQUIRE(ver == 2 && (bn == 0 || bn == 160), "two accumulators: CTA-pair kernel, BLOCK_N 160");
+  if (nsub == 2) bn = 160;
+  // a tap-reuse stage holds the full weight tiles of three taps: BLOCK_N 256 or two accumulators leave no room for two
+  // stages in 227 KB, so the automatic plan falls back to per-tap loads there
+  if (reuse && bn && stages_for(bn, nsub, true, epi_bytes) < 2) {
+    SDW_REQUIRE(d.tr != 2, "tap reuse with this BLOCK_N / accumulator count does not fit two pipeline stages");
+    reuse = false;
+    p.bw = bw = std::min(pow2_floor(Wd), BM);
+    p.bh = bh = std::min(pow2_floor(Hd), BM / bw);
+    p.bb = bb = BM / (bw * bh);
+    p.tiles_w = (Wd + bw - 1) / bw;
+    p.tiles_h = (Hd + bh - 1) / bh;
+    L->tr = 0;
+  }
+  const int m_tiles_f = p.tiles_w * p.tiles_h * ((d.B + bb - 1) / bb);
+  if (bn == 0) {
+    static const int cand1[4] = {256, 160, 128, 64};
+    static const int cand2[4] = {256, 192, 160, 128};
+    const int* cand = ver == 2 ? cand2 : cand1;
+    double best = 1e30;
+    const int groups = (m_tiles_f + CL - 1) / CL;
+    for (int i = 0; i < 4; ++i) {
+      const int c = cand[i];
+      if (d.mode == GEMM_GEGLU && c % 64 != 0) continue;
+      if (stages_for(c, 1, reuse, epi_bytes) < 2) continue;
+      const int tiles = groups * ((d.N + c - 1) / c);
+      const int waves = (tiles + nsm / CL - 1) / (nsm / CL);
+      double cost = static_cast<double>(waves) * c;
+      if (stages_for(c, 1, reuse, epi_bytes) < 3) cost *= 1.6;  // H100: two-stage tap-reuse plans measured ~1.3-1.5x slower per column
+      if (cost < best) {
+        best = cost;
+        bn = c;
       }
     }
-    bn = best_bn;
-  }
-  if (bn == 0) {
-    if (d.mode == GEMM_GEGLU) bn = 128;
-    else if (d.N % 160 == 0 && d.N % 128 != 0) bn = 160;
-    else if (d.N <= 64) bn = 64;
-    else bn = 128;
   }
   SDW_REQUIRE(bn == 64 || bn == 128 || bn == 160 || bn == 256 || (bn == 192 && ver == 2), "unsupported BLOCK_N");
-  if (ver == 2) SDW_REQUIRE(bn != 64, "the 2-CTA kernel needs BLOCK_N >= 128");
+  if (ver == 2) SDW_REQUIRE(bn != 64, "the CTA-pair kernel needs BLOCK_N >= 128");
+  if (d.ew == 4) SDW_REQUIRE(false, "one epilogue form on this GPU: epilogue width 4 is not available");
+  SDW_REQUIRE(d.ew == 0 || d.ew == 2, "epilogue width must be 0 (auto) or 2");
+  L->ew = 2;
   L->ver = ver;
   L->nsub = nsub;
+  L->bn = bn;
   if (d.mode == GEMM_GEGLU) SDW_REQUIRE(bn % 64 == 0 && d.N % 64 == 0, "GEGLU needs 64-column pairs");
   if (d.mode == GEMM_QKV_VT) SDW_REQUIRE(d.vt && d.vt_col0 % 32 == 0 && d.vt_d > 0, "bad V^T split");
-  L->bn = bn;
-  L->grid = dim3(m_tiles_f, (d.N + bn - 1) / bn, 1);
+  p.nstages = stages_for(bn, nsub, reuse, epi_bytes);
+  SDW_REQUIRE(p.nstages >= 2, "no room for a two-stage operand pipeline");
+  p.m_groups = (m_tiles_f + CL - 1) / CL;
+  p.n_tiles = (d.N + bn * nsub - 1) / (bn * nsub);
   {
-    // store staging pays off when the epilogue, not the mainloop, bounds the tile (short K, wide N)
-    static const int stage_env = [] { const char* e = std::getenv("SDW_STAGE"); return e ? std::atoi(e) : -1; }();
-    const int kblocks = p.ntaps * kchunks;
-    p.stage_stores = stage_env >= 0 ? stage_env : (kblocks <= 10 && d.N >= 640 ? 1 : 0);
-    // the coalescing stage keeps 32-bit row offsets
-    const int64_t max_off = static_cast<int64_t>(d.B) * OH * OW * std::max<int64_t>(d.ldc, d.ldr ? d.ldr : d.ldc);
-    SDW_REQUIRE(max_off < (int64_t(1) << 31) || ver == 1, "output too large for the 2-CTA epilogue (>= 2^31 elements)");
-  }
-  L->ew = 2;
-  if (ver == 2) {
-    p.m_pairs = (m_tiles_f + 1) / 2;
-    p.n_tiles = (d.N + bn * nsub - 1) / (bn * nsub);
-    L->grid = dim3(2 * std::min(p.m_pairs * p.n_tiles, 74), 1, 1);  // one CTA pair per SM pair
-    // division-free tile coordinates (sdw_gemm2.cu: tile_coords)
-    {
-      const int n_groups = p.n_tiles;
-      const int64_t max_t = static_cast<int64_t>(p.m_pairs) * n_groups, max_m = 2 * static_cast<int64_t>(p.m_pairs) + 1;
-      auto magic = [](int64_t dv) { return dv <= 1 ? 0u : static_cast<uint32_t>(((int64_t(1) << 32) + dv - 1) / dv); };
-      const int64_t twh = static_cast<int64_t>(p.tiles_w) * p.tiles_h;
-      SDW_REQUIRE(max_t * n_groups < (int64_t(1) << 32) && max_m * twh < (int64_t(1) << 32), "tile grid too large for the 32-bit fast division");
-      p.mg_ng = magic(n_groups);
-      p.mg_tw = magic(p.tiles_w);
-      p.mg_twh = magic(twh);
-    }
+    const int64_t total = static_cast<int64_t>(p.m_groups) * p.n_tiles;
+    SDW_REQUIRE(total < (int64_t(1) << 31), "tile grid too large");
+    L->grid = dim3(static_cast<unsigned>(CL * std::min<int64_t>(total, nsm / CL)), 1, 1);  // persistent
   }
   {
     auto lg2 = [](int v) { int l = 0; while ((1 << l) < v) ++l; return l; };
@@ -435,88 +722,26 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
                            static_cast<uint64_t>(d.b_batched ? d.sBb : 0)};
     for (int i = 2; i < 4; ++i)
       if (strides[i] == 0) strides[i] = static_cast<uint64_t>(ldb);
-    uint32_t box[4] = {BK, static_cast<uint32_t>(ver == 2 ? bn / 2 : bn), 1, 1};
+    uint32_t box[4] = {BK, static_cast<uint32_t>(bn / CL), 1, 1};
     if (int e = encode_map(&p.mapB, d.Wt, 4, dims, strides, box)) return e;
   }
-  // ---- epilogue flavour and pipeline depth of the 2-CTA kernel ----------------------------------------------------
-  p.epi_tma = 0;
-  p.nstages = 0;
-  if (ver == 2) {
-    const int64_t osW = d.o_sW || d.o_sH || d.o_sB ? d.o_sW : d.ldc;
-    const int64_t osH = d.o_sW || d.o_sH || d.o_sB ? d.o_sH : OW * d.ldc;
-    const int64_t osB = d.o_sW || d.o_sH || d.o_sB ? d.o_sB : OH * OW * d.ldc;
-    const int64_t ldr = d.ldr ? d.ldr : d.ldc;
-    const int64_t rsW = d.r_sW || d.r_sH || d.r_sB ? d.r_sW : ldr;
-    const int64_t rsH = d.r_sW || d.r_sH || d.r_sB ? d.r_sH : OW * ldr;
-    const int64_t rsB = d.r_sW || d.r_sH || d.r_sB ? d.r_sB : OH * OW * ldr;
-    auto ok16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
-    auto ok_strides = [&](int64_t sw, int64_t sh, int64_t sb) {
-      return sw > 0 && sw % 8 == 0 && (Hd == 1 || sh % 8 == 0) && (d.B == 1 || sb % 8 == 0);
-    };
-    const int ncols = d.mode == GEMM_GEGLU ? d.N / 2 : (d.mode == GEMM_QKV_VT ? d.vt_col0 : d.N);
-    // V^T scatter through TMA: token lattice (H == 1, 128-token tiles), 32-column chunks never straddle vt_col0
-    const bool vt_ok = d.mode != GEMM_QKV_VT ||
-                       (Hd == 1 && bw == BM && d.conv == 0 && d.vt_col0 % 32 == 0 && d.vt_ld % 8 == 0 && ok16(d.vt) &&
-                        d.vt_ntok == Wd && !d.resid);
-    bool can = nsub == 1 && !d.b_batched && vt_ok && (!d.rowvec || d.rowvec_ld == 0) &&
-               d.N % 8 == 0 && bn <= 256 && ok16(d.out) && ok_strides(osW, osH, osB) && (!d.bias || ok16(d.bias)) &&
-               (!d.resid || (ok16(d.resid) && ok_strides(rsW, rsH, rsB) && d.mode == GEMM_PLAIN));
-    if (d.et == 2) SDW_REQUIRE(can, "the TMA epilogue needs the CTA-pair kernel, plain/GEGLU mode, no row vector and 16-byte aligned views");
-    static const int et_env = [] { const char* e = std::getenv("SDW_EPI_TMA"); return e ? std::atoi(e) : -1; }();
-    const int kblocks = p.ntaps * kchunks;
-    // short-K GEMMs are bound by their epilogue (profiles/r01_ncu_epilogue_shortk.md) and gain up to 2x; long-K ones
-    // lose one operand stage to the epilogue buffers but still come out ahead end to end (bench: 8.49 -> 8.56 frames/s),
-    // so the TMA epilogue is used wherever it is eligible.  SDW_EPI_TMA=0 disables it, =2 restricts it to <= 24 K blocks.
-    const bool want = d.et == 2 || (d.et == 0 && (et_env < 0 || et_env == 1 || (et_env == 2 && kblocks <= 24)));
-    p.epi_tma = can && want ? 1 : 0;
-    const int a_stage = reuse ? 20480 : 16384;
-    const int b_stage = (reuse ? 3 : 1) * nsub * (bn / 2) * 128;
-    const int epi_bytes = p.epi_tma ? G2_EPI_OUT + G2_EPI_BIAS + (d.resid ? G2_RES_STAGES * G2_RES_STAGE : 0) : G2_EPI_OLD;
-    p.nstages = std::min(8, (G2_SMEM_USABLE - G2_BAR_BYTES - epi_bytes) / (a_stage + b_stage));
-    SDW_REQUIRE(p.nstages >= 2, "no room for a two-stage operand pipeline");
-    // epilogue width: four warps per TMEM lane quarter where the epilogue, not the MMA, sets the tile time — K <= 448
-    // (the 64x64-level transformer linears, K = 320: GEGLU 434 -> 383 us, QKV-like 218 -> 161 us, out-projection 99 ->
-    // 88 us at batch 60, same box; from K = 640 on the MMA is the longer leg and the wider epilogue loses 2-10 %:
-    // profiles/r02_epilogue_width_ab_same_box.txt).  SDW_GEMM_EW=2 | 4: 8-warp epilogue everywhere / 16 wherever eligible
-    {
-      static const int ew_env = [] { const char* e = std::getenv("SDW_GEMM_EW"); return e ? std::atoi(e) : 0; }();
-      const bool can4 = p.epi_tma && nsub == 1 && !reuse;
-      if (d.ew == 4) SDW_REQUIRE(can4, "the 16-warp epilogue needs the TMA epilogue, one accumulator and the per-tap mainloop");
-      const int want4 = d.ew ? d.ew == 4 : (ew_env ? ew_env == 4 : kblocks <= 7);
-      L->ew = can4 && want4 ? 4 : 2;
-      if (L->ew == 4) {  // 16 per-warp bias copies instead of 8, eight residual ring slots instead of four
-        const int extra = G2_EPI_BIAS + (d.resid ? G2_RES_STAGES * G2_RES_STAGE : 0);
-        p.nstages = std::min(8, (G2_SMEM_USABLE - G2_BAR_BYTES - epi_bytes - extra) / (a_stage + b_stage));
-        SDW_REQUIRE(p.nstages >= 2, "no room for a two-stage operand pipeline");
-      }
-    }
-    if (p.epi_tma) {
-      // output lattice: column, then the tile lattice (w, h, b) with the parity scatter folded into base + strides
-      const int sw_ = std::min(bw, 32), sh_ = std::min(bh, 32 / sw_), sb_ = 32 / (sw_ * sh_);
-      uint64_t dims[4] = {static_cast<uint64_t>(ncols), static_cast<uint64_t>(Wd), static_cast<uint64_t>(Hd),
-                          static_cast<uint64_t>(d.B)};
-      auto fix = [&](uint64_t* st) {  // extents of one still need a legal stride
-        for (int i = 2; i < 4; ++i)
-          if (st[i] == 0 || st[i] % 8 != 0) st[i] = st[1] * static_cast<uint64_t>(Wd);
-      };
-      uint64_t so[4] = {1, static_cast<uint64_t>(osW * p.os), static_cast<uint64_t>(osH * p.os), static_cast<uint64_t>(osB)};
-      fix(so);
-      uint32_t box_o[4] = {32, static_cast<uint32_t>(sw_), static_cast<uint32_t>(sh_), static_cast<uint32_t>(sb_)};
-      if (int e = encode_map(&p.mapOut, d.out + p.oy * osH + p.ox * osW, 4, dims, so, box_o, 64)) return e;
-      if (d.mode == GEMM_QKV_VT) {
-        const int vrows = d.N - d.vt_col0;  // heads * d rows of V^T per sample
-        uint64_t dv[3] = {static_cast<uint64_t>(Wd), static_cast<uint64_t>(vrows), static_cast<uint64_t>(d.B)};
-        uint64_t sv[3] = {1, static_cast<uint64_t>(d.vt_ld), static_cast<uint64_t>(d.vt_ld) * static_cast<uint64_t>(d.vt_heads) * d.vt_d};
-        uint32_t bv[3] = {32, 32, 1};
-        SDW_REQUIRE(vrows == d.vt_heads * d.vt_d, "V^T rows must be heads x d");
-        if (int e = encode_map(&p.mapVt, d.vt, 3, dv, sv, bv, 0)) return e;
-      }
-      if (d.resid) {
-        uint64_t sr[4] = {1, static_cast<uint64_t>(rsW * p.os), static_cast<uint64_t>(rsH * p.os), static_cast<uint64_t>(rsB)};
-        fix(sr);
-        uint32_t box_r[4] = {32, static_cast<uint32_t>(bw), static_cast<uint32_t>(bh), static_cast<uint32_t>(bb)};
-        if (int e = encode_map(&p.mapRes, d.resid + p.oy * rsH + p.ox * rsW, 4, dims, sr, box_r, 64)) return e;
-      }
+  if (p.epi_tma) {
+    // output lattice: column, then the tile lattice (w, h, b) with the parity scatter folded into base + strides; the
+    // box is one consumer warpgroup's 64 rows x 32 columns
+    const int hw = std::min(bw, 64), hh = std::min(bh, 64 / hw), hb = 64 / (hw * hh);
+    uint64_t dims[4] = {static_cast<uint64_t>(ncols), static_cast<uint64_t>(Wd), static_cast<uint64_t>(Hd),
+                        static_cast<uint64_t>(d.B)};
+    uint64_t so[4] = {1, static_cast<uint64_t>(osW * p.os), static_cast<uint64_t>(osH * p.os), static_cast<uint64_t>(osB)};
+    for (int i = 2; i < 4; ++i)  // extents of one still need a legal stride
+      if (so[i] == 0 || so[i] % 8 != 0) so[i] = so[1] * static_cast<uint64_t>(Wd);
+    uint32_t box[4] = {32, static_cast<uint32_t>(hw), static_cast<uint32_t>(hh), static_cast<uint32_t>(hb)};
+    if (int e = encode_map(&p.mapOut, d.out + p.oy * osH + p.ox * osW, 4, dims, so, box, 0)) return e;
+    if (d.resid) {
+      uint64_t sr[4] = {1, static_cast<uint64_t>(res_sW * p.os), static_cast<uint64_t>(res_sH * p.os),
+                        static_cast<uint64_t>(res_sB)};
+      for (int i = 2; i < 4; ++i)
+        if (sr[i] == 0 || sr[i] % 8 != 0) sr[i] = sr[1] * static_cast<uint64_t>(Wd);
+      if (int e = encode_map(&p.mapRes, d.resid + p.oy * res_sH + p.ox * res_sW, 4, dims, sr, box, 0)) return e;
     }
   }
   p.bias = d.bias;
@@ -524,17 +749,15 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
   p.rowvec_ld = d.rowvec_ld;
   p.resid = d.resid;
   p.out = d.out;
-  if (d.o_sW || d.o_sH || d.o_sB) {
-    p.o_sW = d.o_sW; p.o_sH = d.o_sH; p.o_sB = d.o_sB;
-  } else {
-    p.o_sW = d.ldc; p.o_sH = OW * d.ldc; p.o_sB = OH * OW * d.ldc;
-  }
-  if (d.r_sW || d.r_sH || d.r_sB) {
-    p.r_sW = d.r_sW; p.r_sH = d.r_sH; p.r_sB = d.r_sB;
-  } else {
-    const int64_t ldr = d.ldr ? d.ldr : d.ldc;
-    p.r_sW = ldr; p.r_sH = OW * ldr; p.r_sB = OH * OW * ldr;
-  }
+  p.o_sW = osW;
+  p.o_sH = osH;
+  p.o_sB = osB;
+  p.r_sW = res_sW;
+  p.r_sH = res_sH;
+  p.r_sB = res_sB;
+  // two-column (4-byte) output / residual accesses: every row offset and the column pair start even
+  p.vec2 = ((p.o_sW | p.o_sH | p.o_sB) & 1) == 0 && (reinterpret_cast<uintptr_t>(d.out) & 3) == 0 &&
+           (!d.resid || (((p.r_sW | p.r_sH | p.r_sB) & 1) == 0 && (reinterpret_cast<uintptr_t>(d.resid) & 3) == 0));
   p.mode = d.mode;
   p.act = d.act;
   p.alpha = d.alpha;
@@ -547,27 +770,61 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
   return 0;
 }
 
-int launch_gemm(const GemmLaunch& l, cudaStream_t stream) {
-  if (l.ver == 2) return launch_gemm2(l, stream);
-  switch (l.bn) {
-    case 64:
-      SDW_CUDA_OK(launch_pdl(gemm_tc_kernel<64>, l.grid, dim3(GEMM_THREADS), GemmCfg<64>::SMEM_BYTES, stream, l.p));
-      break;
-    case 128:
-      SDW_CUDA_OK(launch_pdl(gemm_tc_kernel<128>, l.grid, dim3(GEMM_THREADS), GemmCfg<128>::SMEM_BYTES, stream, l.p));
-      break;
-    case 160:
-      SDW_CUDA_OK(launch_pdl(gemm_tc_kernel<160>, l.grid, dim3(GEMM_THREADS), GemmCfg<160>::SMEM_BYTES, stream, l.p));
-      break;
-    case 256:
-      SDW_CUDA_OK(launch_pdl(gemm_tc_kernel<256>, l.grid, dim3(GEMM_THREADS), GemmCfg<256>::SMEM_BYTES, stream, l.p));
-      break;
-    default:
-      set_error("bad BLOCK_N");
-      return 1;
+template <int BN, int NSUB, int TR, int CL>
+static int launch_one(const GemmLaunch& l, cudaStream_t stream) {
+  static int max_ctas = 0;  // CTAs of this kernel that can be resident at once (whole clusters)
+  if (!max_ctas) {
+    SDW_CUDA_OK(cudaFuncSetAttribute(gemm_kernel<BN, NSUB, TR, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     GEMM_SMEM_DYN));
+    max_ctas = sm_count();
+    if (CL > 1) {
+      // clusters must fit inside one GPC: fewer than SMs / CL of them may be co-resident, and a persistent grid larger
+      // than that would run its last clusters as a second wave
+      cudaLaunchConfig_t cfg{};
+      cfg.gridDim = dim3(CL * (sm_count() / CL));
+      cfg.blockDim = dim3(GEMM_THREADS);
+      cfg.dynamicSmemBytes = GEMM_SMEM_DYN;
+      cudaLaunchAttribute attr[1];
+      attr[0].id = cudaLaunchAttributeClusterDimension;
+      attr[0].val.clusterDim.x = CL;
+      attr[0].val.clusterDim.y = 1;
+      attr[0].val.clusterDim.z = 1;
+      cfg.attrs = attr;
+      cfg.numAttrs = 1;
+      int nclusters = 0;
+      SDW_CUDA_OK(cudaOccupancyMaxActiveClusters(&nclusters, gemm_kernel<BN, NSUB, TR, CL>, &cfg));
+      if (nclusters > 0) max_ctas = std::min(max_ctas, CL * nclusters);
+    }
   }
+  const dim3 grid(std::min<unsigned>(l.grid.x, static_cast<unsigned>(max_ctas)), 1, 1);
+  SDW_CUDA_OK(launch_cluster(gemm_kernel<BN, NSUB, TR, CL>, grid, dim3(GEMM_THREADS), GEMM_SMEM_DYN, stream, CL, l.p));
   SDW_CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+// instantiations: single CTAs with BLOCK_N 64 / 128 / 160 / 256; CTA pairs with BLOCK_N 128 / 160 / 192 / 256 x
+// {per-tap, tap reuse} and one accumulator, 160 x 2 accumulators
+int launch_gemm(const GemmLaunch& l, cudaStream_t stream) {
+  const int key = l.ver * 100000 + l.bn * 100 + l.nsub * 10 + (l.tr ? 1 : 0);
+  switch (key) {
+    case 106410: return launch_one<64, 1, 0, 1>(l, stream);
+    case 112810: return launch_one<128, 1, 0, 1>(l, stream);
+    case 116010: return launch_one<160, 1, 0, 1>(l, stream);
+    case 125610: return launch_one<256, 1, 0, 1>(l, stream);
+    case 212810: return launch_one<128, 1, 0, 2>(l, stream);
+    case 216010: return launch_one<160, 1, 0, 2>(l, stream);
+    case 219210: return launch_one<192, 1, 0, 2>(l, stream);
+    case 225610: return launch_one<256, 1, 0, 2>(l, stream);
+    case 216020: return launch_one<160, 2, 0, 2>(l, stream);
+    case 212811: return launch_one<128, 1, 1, 2>(l, stream);
+    case 216011: return launch_one<160, 1, 1, 2>(l, stream);
+    case 219211: return launch_one<192, 1, 1, 2>(l, stream);
+    case 225611: return launch_one<256, 1, 1, 2>(l, stream);
+    case 216021: return launch_one<160, 2, 1, 2>(l, stream);
+    default: break;
+  }
+  set_error("no GEMM kernel for this version / BLOCK_N / accumulators / tap reuse combination");
+  return 1;
 }
 
 }  // namespace sdw

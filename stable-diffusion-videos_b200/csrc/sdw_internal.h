@@ -51,9 +51,38 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
+// the same, as clusters of `cluster` CTAs along x
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                              int cluster, Args&&... args) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[2];
+  int n = 0;
+  attr[n].id = cudaLaunchAttributeClusterDimension;
+  attr[n].val.clusterDim.x = cluster;
+  attr[n].val.clusterDim.y = 1;
+  attr[n].val.clusterDim.z = 1;
+  ++n;
+  if (pdl_enabled()) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
+  cfg.attrs = attr;
+  cfg.numAttrs = n;
+  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
+// number of SMs of the current device (H100_SMS in plan-only mode)
+constexpr int H100_SMS = 132;
+int sm_count();
 
 // ---------------------------------------------------------------------------
-// tcgen05 implicit-GEMM (conv3x3 / conv1x1 / linear / batched matmul)
+// wgmma implicit-GEMM (conv3x3 / conv1x1 / linear / batched matmul)
 // ---------------------------------------------------------------------------
 // out[pix, n] = epi( sum_{tap, c} A[lattice(tap)][pix shifted by (dx,dy)][c] * Wt[n][tap*Cp + c] )
 // A is an NHWC fp16 lattice (C, W, H, B) read through up to four TMA maps (one
@@ -67,28 +96,20 @@ enum GemmMode : int {
 struct alignas(64) GemmKParams {
   CUtensorMap mapA[4];
   CUtensorMap mapB;
+  CUtensorMap mapOut;       // TMA epilogue: (columns, w, h, b) lattice of the output, box (32, 64 rows of the tile)
+  CUtensorMap mapRes;       // ... of the residual, same box
   int8_t tap_map[12], tap_dx[12], tap_dy[12];
   int ntaps, kchunks;       // K blocks = ntaps * kchunks, each 64 wide
   int W, H, B;              // tile-grid domain (the A lattice extents)
-  int bw, bh, bb;           // M tile = bw*bh*bb = 128 lattice points
-  int tiles_w, tiles_h;     // tiles per (w,h); tiles along b = gridDim.x / (tiles_w*tiles_h)
-  // 2-CTA kernel: tile coordinates without integer divisions (7 per tile per warp used to be a quarter of the epilogue's
-  // instruction stream on short-K GEMMs: profiles/r02_ncu_epilogue_shortk.md).  bw, bh, bb are powers of two (shifts);
-  // n_groups, tiles_w, tiles_w * tiles_h go through q = umulhi(n, ceil(2^32 / d)), exact for n * d < 2^32 (planner-checked)
+  int bw, bh, bb;           // M tile = bw*bh*bb = 128 lattice points (powers of two)
   int lg_bw, lg_bh;
-  uint32_t mg_ng, mg_tw, mg_twh;  // 0 = divisor 1
+  int tiles_w, tiles_h;     // tiles per (w,h)
+  int m_groups, n_tiles;    // persistent tile grid: groups of CL vertically adjacent 128-row M tiles x N tiles
   int N;                    // GEMM N (packed columns)
   int b_batched;            // 1: weight map coords (.., y0, b0) = lattice (h, b) (batched matmul)
-  int stage_stores;         // 1: bounce output chunks through shared memory for coalesced stores (wide-N GEMMs)
-  int m_pairs, n_tiles;     // 2-CTA persistent kernel: tile grid (pairs of 128-row M tiles x BN-wide N tiles)
-  int tap_reuse;            // 1: 3x3 conv with one (bh+2)-row activation box per (channel chunk, kx) shared by the 3 ky taps
-  // TMA epilogue (2-CTA kernel, short-K GEMMs): output chunks leave through TMA stores, the residual tile arrives
-  // through a TMA-fed shared-memory ring, the bias is staged per warp (sdw_gemm_epi.cuh: gemm_epilogue_tma)
-  CUtensorMap mapOut;       // (columns, w, h, b) lattice of the output, box (32, slab_w, slab_h, slab_b), 64B swizzle
-  CUtensorMap mapRes;       // ... of the residual, box (32, bw, bh, bb)
-  CUtensorMap mapVt;        // GEMM_QKV_VT: V^T as (token, head * d + dd, sample), box (32 tokens, 32 rows), no swizzle
-  int epi_tma;
+  int epi_tma;              // 1: output chunks staged in shared memory and written by TMA stores
   int nstages;              // mainloop pipeline depth (what the epilogue buffers leave of the 227 KB)
+  int vec2;                 // 1: output / residual rows allow 4-byte column-pair accesses
   // epilogue
   const float* bias;        // [N] or null
   const float* rowvec;      // [B][rowvec_ld] per-sample vector added per column (time-embedding proj) or null
@@ -110,11 +131,11 @@ struct alignas(64) GemmKParams {
 struct GemmLaunch {
   GemmKParams p;
   dim3 grid;
-  int bn;   // BLOCK_N variant
-  int ver;  // 1: one 128xBN tile per CTA (sdw_gemm.cu); 2: persistent CTA pairs, 256xBN tiles (sdw_gemm2.cu)
-  int nsub = 1;  // ver 2: accumulators per activation tile (2 -> 256 x 2*BN tiles, single-buffered TMEM)
-  int ew = 2;    // ver 2: epilogue warps per TMEM lane quarter (4 -> the 640-thread kernel for epilogue-bound short-K GEMMs)
-  int tr = 0;    // ver 2: 1 -> tap-reuse mainloop (3x3 stride-1 convs; GemmKParams::tap_reuse)
+  int bn;        // BLOCK_N variant
+  int ver;       // 1: single CTAs; 2: CTA pairs (clusters of two) sharing each weight tile through TMA multicast
+  int nsub = 1;  // accumulators per activation tile (2 -> 128 x 2*BN tiles)
+  int ew = 2;    // epilogue warps per 32 accumulator rows (always 2: each consumer warpgroup stores its own rows)
+  int tr = 0;    // 1 -> tap-reuse mainloop (3x3 stride-1 convs)
 };
 
 // Describes one implicit GEMM in host terms; plan_gemm() turns it into a launch.
@@ -148,26 +169,22 @@ struct GemmDesc {
   int64_t vt_ld = 0;
   int bn = 0;   // 0 = auto
   int ver = 0;  // 0 = auto, 1 / 2 force a kernel version
-  int nsub = 0; // 0 = auto, 1 / 2: accumulators per activation tile in the 2-CTA kernel
-  int ew = 0;   // 0 = auto, 2 / 4: epilogue warps per TMEM lane quarter in the 2-CTA kernel (4 needs the TMA epilogue)
-  int tr = 0;   // 0 = auto, 1 = never, 2 = require the tap-reuse mainloop (3x3 stride-1 conv, W % 16 == 0, H % 8 == 0)
-  int et = 0;   // 0 = auto, 1 = never, 2 = require the TMA epilogue
+  int nsub = 0; // 0 = auto, 1 / 2: accumulators per activation tile (2: CTA-pair kernel, BLOCK_N 160)
+  int ew = 0;   // 0 = auto or 2 (the only epilogue width of this kernel)
+  int tr = 0;   // 0 = auto, 1 = never, 2 = require the tap-reuse mainloop (3x3 stride-1 conv, W % 16 == 0, H % 8 == 0, CTA pairs)
+  int et = 0;   // 0 = auto, 1 = never, 2 = require the TMA-store epilogue
 };
 
 int plan_gemm(const GemmDesc& d, GemmLaunch* out);
 int launch_gemm(const GemmLaunch& l, cudaStream_t stream);
-int launch_gemm2(const GemmLaunch& l, cudaStream_t stream);
-int gemm2_init();
 void set_plan_only(bool on);
-int gemm_init();  // resolves the driver entry point, sets smem attributes
-// shared-memory budget of the 2-CTA kernel (sdw_gemm2.cu): barriers, then the operand ring, then the epilogue buffers
-constexpr int G2_SMEM_DYN = 227 * 1024;                    // requested dynamic shared memory
-constexpr int G2_SMEM_USABLE = G2_SMEM_DYN - 1024;         // after the 1 KB alignment slack
-constexpr int G2_BAR_BYTES = 1024;
-constexpr int G2_EPI_OLD = 8 * 2048;                       // 2 KB store-coalescing buffer per epilogue warp
-constexpr int G2_EPI_OUT = 8 * 2 * 2048;                   // TMA epilogue: 32-row x 64-byte output slabs, two per warp (8 warps) or one (16)
-constexpr int G2_EPI_BIAS = 8 * 1024;                      //   per-warp bias copy (<= 256 fp32 columns); twice that for 16 warps
-constexpr int G2_RES_STAGES = 4, G2_RES_STAGE = 128 * 64;  //   residual ring: [128 rows x 32 columns] fp16 chunks, 4 slots (8 with 16 epilogue warps)
+int gemm_init();  // resolves the driver entry point of the tensor-map encoder
+// shared-memory budget of the GEMM kernel: barriers, then the operand ring, then the epilogue buffers
+constexpr int GEMM_SMEM_DYN = 227 * 1024;                  // requested dynamic shared memory (the sm_90 maximum)
+constexpr int GEMM_SMEM_USABLE = GEMM_SMEM_DYN - 1024;     // after the 1 KB alignment slack
+constexpr int GEMM_BAR_BYTES = 1024;
+constexpr int GEMM_MAX_STAGES = 8;
+constexpr int GEMM_EPI_BYTES = 2 * 2 * 4096;               // TMA epilogue: two 64-row x 32-column fp16 buffers per warpgroup
 int encode_map(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_elems,
                const uint32_t* box, int swizzle_bytes = 128);
 
@@ -192,7 +209,6 @@ bool attn_supported(int d);
 int plan_attention(const AttnDesc& a, AttnLaunch* L);
 int launch_attention(const AttnLaunch& L, cudaStream_t stream);
 void attention_plan_info(const AttnLaunch& L, int out[5]);
-void attention_set_trace(long long* buf);  // device buffer [2][4096][8] of clock64 stamps written by CTA 0 of attn_pp_kernel (nullptr = off)
 
 // ---------------------------------------------------------------------------
 // fp32 helper kernels (sdw_elem.cu)

@@ -220,10 +220,6 @@ __global__ void __launch_bounds__(256, 3) gn_apply_kernel(const __half* __restri
   }
 }
 
-// (A single-launch variant — one thread-block cluster per sample, statistics exchanged through distributed shared memory,
-//  the slice normalised while still in L2 — was built, measured slower (64x64x320, batch 32: 130 us vs 82 us; VAE
-//  512x512x128: 2.1 ms vs 0.82 ms: 18 clusters of 8 CTAs keep too few loads in flight) and removed.)
-
 // back-to-front block order of the statistics / LayerNorm passes (L2 reuse of the producer's output); SDW_NORM_REV=0 = A/B
 int norm_reverse() {
   static const int v = [] { const char* e = std::getenv("SDW_NORM_REV"); return e ? std::atoi(e) : 1; }();
@@ -232,7 +228,7 @@ int norm_reverse() {
 
 // chunks per sample: enough blocks to fill the machine (B * nchunks >= ~4 waves) while keeping >= 16 pixels each
 int gn_chunks(int64_t P, int B) {
-  int64_t want = (148 * 7 + B - 1) / B;  // 7 blocks of the stats kernel fit an SM (30 KB of shared memory each)
+  int64_t want = (static_cast<int64_t>(sm_count()) * 7 + B - 1) / B;  // 7 blocks of the stats kernel fit an SM (30 KB of shared memory each)
   int64_t n = std::min<int64_t>(want, P / 16);
   if (n < 1) n = 1;
   if (n > GN_MAX_CHUNKS) n = GN_MAX_CHUNKS;
@@ -260,9 +256,8 @@ int groupnorm(const __half* x, int64_t ldx, int B, int64_t P, int C, int G, cons
   const int BG = B * G;
   SDW_CUDA_OK(launch_pdl(gn_finalize_kernel, dim3((BG + 7) / 8), dim3(256), 0, stream, partial_ws, nchunks, G, BG,
                          static_cast<float>(P) * (C / G), eps, stats));
-  // one full wave: 148 SMs x 8 resident 256-thread blocks, split evenly over the samples (the former fixed ~100-pixel
-  // tiles gave 1376 blocks = 1.16 waves at 64x64x320, batch 32: the second wave ran 16 % full)
-  const int64_t per_sample = std::max<int64_t>(1, (148 * 3) / B);  // 3 resident blocks per SM (launch bounds)
+  // one full wave of resident blocks, split evenly over the samples
+  const int64_t per_sample = std::max<int64_t>(1, (static_cast<int64_t>(sm_count()) * 3) / B);  // 3 resident blocks per SM (launch bounds)
   const int ppb = static_cast<int>(std::max<int64_t>(1, (P + per_sample - 1) / per_sample));
   const unsigned tiles = static_cast<unsigned>((P + ppb - 1) / ppb);
   SDW_CUDA_OK(launch_pdl(gn_apply_kernel, dim3(tiles, B), dim3(256), static_cast<size_t>(2) * C * sizeof(float), stream, x, ldx,
@@ -357,11 +352,9 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const __half* __restrict
 
 // LayerNorm for C = 40 * LPR (320 / 640 / 1280: every width of the SD UNets): LPR lanes share a row, five 16-byte vectors
 // per lane, so all 32 lanes carry data (the generic kernel runs its second vector slot 25 % full at C = 320), the
-// reductions stay inside LPR-lane groups, the arithmetic is packed fp32x2 and gamma / beta come from shared memory.
-// ncu on the generic kernel at C = 320: issue slots 65 % busy at 34 % occupancy and 37 % of the DRAM peak — it was bound
-// by its instruction count (~200 per 16-byte vector), not by HBM (profiles/r02_ncu_norms.txt).
-// (A persistent "streaming" form of the generic kernel — fixed grid, next row group's loads in flight — was measured
-//  SLOWER, 112 vs 87 us at C = 320, and dropped: the loads were never the problem.)
+// reductions stay inside LPR-lane groups, the arithmetic runs on fp32 pairs and gamma / beta come from shared memory:
+// far fewer instructions per 16-byte vector than the generic kernel, which is bound by its instruction count rather
+// than by HBM at these widths.
 template <int LPR, int ITER>
 __global__ void __launch_bounds__(256) layernorm_c40_kernel(const __half* __restrict__ x, int64_t ldx, int64_t rows,
                                                             const float* __restrict__ gamma,
@@ -563,7 +556,7 @@ __global__ void __launch_bounds__(512) conv_in_kernel(const __half* __restrict__
                                                        int N, __half* __restrict__ y, int64_t ldy,
                                                        int pix_per_block) {
   // patch[pair][k] = (x of pixel 2*pair, x of pixel 2*pair + 1) for the 9*CIN taps: one 16-byte broadcast read feeds two
-  // packed FMAs (two taps x two pixels); thread = output channel, its 9*CIN weights live in registers
+  // FMAs on fp32 pairs (two taps x two pixels); thread = output channel, its 9*CIN weights live in registers
   constexpr int K = 9 * CIN;
   extern __shared__ float2 patch2[];  // [pix_per_block / 2][K]
   const int64_t P = static_cast<int64_t>(B) * H * W;
@@ -633,7 +626,7 @@ int conv_in_small(const __half* x, int64_t ldx, int B, int H, int W, int Cin, co
 //   out_u8   : uint8 NHWC [P][NOUT] = round(clamp(v/2+0.5,0,1)*255) (VAE frame; P:435-438 + numpy_to_pil) — optional
 // =============================================================================================
 // A block owns a TS x TS pixel tile: its (TS+2)^2 halo is staged once in shared memory (the row-per-warp version
-// re-read every input pixel nine times from L2: 245 us for the UNet's 320->4 conv, ~6 ms for the VAE's 128->3), the
+// re-read every input pixel nine times from L2), the
 // weights sit next to it; a warp computes 8 pixels at a time, lanes split the channels, one tap's weights in registers.
 template <int NOUT, int TS>
 __global__ void __launch_bounds__(256) conv_out_kernel(const __half* __restrict__ x, int64_t ldx, int B, int H, int W,
@@ -771,7 +764,7 @@ static int launch_conv_out(const __half* x, int64_t ldx, int B, int H, int W, in
     attr_done = true;
   }
   const int64_t tiles = static_cast<int64_t>(B) * ((H + TS - 1) / TS) * ((W + TS - 1) / TS);
-  const int64_t blocks = std::min<int64_t>(tiles, 148 * 2);  // persistent: the weights are staged once per block
+  const int64_t blocks = std::min<int64_t>(tiles, static_cast<int64_t>(sm_count()) * 2);  // persistent: the weights are staged once per block
   conv_out_kernel<NOUT, TS><<<static_cast<unsigned>(blocks), 256, smem, stream>>>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8);
   SDW_CUDA_OK(cudaGetLastError());
   return 0;

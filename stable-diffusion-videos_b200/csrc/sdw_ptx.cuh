@@ -1,14 +1,17 @@
-// sdw_ptx.cuh — inline-PTX wrappers for the Blackwell (sm_100a) primitives the
-// latent-walk kernels are built from: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (TMEM alloc / MMA / commit / ld) and the UMMA descriptors.
+// sdw_ptx.cuh — inline-PTX wrappers for the Hopper (sm_90a) primitives the latent-walk kernels are built from:
+// mbarrier, TMA (cp.async.bulk.tensor, including the cluster multicast form), thread-block clusters, and the
+// warpgroup-MMA (wgmma) fences and shared-memory matrix descriptors.  The wgmma instructions themselves are in
+// sdw_wgmma.cuh.
 //
-// Everything here is device-side plumbing; the kernels live in sdw_gemm.cu
-// (implicit-GEMM conv / linear) and sdw_attn.cu (flash attention).
+// Everything here is device-side plumbing; the kernels live in sdw_gemm.cu (implicit-GEMM conv / linear) and
+// sdw_attn.cu (flash attention).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "sdw_wgmma.cuh"
 
 namespace sdw {
 
@@ -17,18 +20,6 @@ namespace sdw {
 // ----------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ bool elect_one_sync() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ----------------------------------------------------------------------------
@@ -41,7 +32,7 @@ __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() {
-  // make generic-proxy smem writes visible to the async proxy (TMA / UMMA reads)
+  // make generic-proxy smem writes visible to the async proxy (TMA stores read them)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -75,18 +66,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void tma_prefetch_desc(const void* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
-__device__ __forceinline__ void tma_load_2d(const void* map, uint64_t* bar, void* dst, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(const void* map, uint64_t* bar, void* dst, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_4d(const void* map, uint64_t* bar, void* dst, int c0, int c1, int c2,
                                             int c3) {
   asm volatile(
@@ -96,17 +75,23 @@ __device__ __forceinline__ void tma_load_4d(const void* map, uint64_t* bar, void
       "r"(c3)
       : "memory");
 }
+// the same box written to the same shared-memory offset of every CTA in `mask` (cluster multicast); each destination
+// CTA's barrier at the offset of `bar` receives the completion bytes of its copy
+__device__ __forceinline__ void tma_load_4d_mc(const void* map, uint64_t* bar, void* dst, int c0, int c1, int c2, int c3,
+                                               uint16_t mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, "
+      "%4, %5, %6}], [%2], %7;"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
+      "r"(c3), "h"(mask)
+      : "memory");
+}
 
 // TMA store (shared::cta -> global through a tensor map; rows / columns outside the tensor are clipped) and its
 // bulk-group bookkeeping (issued and waited on by the same thread)
 __device__ __forceinline__ void tma_store_4d(const void* map, const void* src, int c0, int c1, int c2, int c3) {
   asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_3d(const void* map, const void* src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
@@ -120,90 +105,7 @@ __device__ __forceinline__ void bulk_wait_group() {
 }
 
 // ----------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, MMA, commit, TMEM loads
-// ----------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]^T ; fp16/bf16 inputs, fp32 accumulate; one thread issues.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]^T : the A operand (M = 128 rows = TMEM lanes, K-major, two fp16 per 32-bit column,
-// 8 columns per K = 16 step) is read from tensor memory — the attention kernel keeps P there instead of bouncing it
-// through shared memory.
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread i = lane i of the warp quarter).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-      "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-
-// ----------------------------------------------------------------------------
-// 2-CTA (cta_group::2) variants: CTA pairs of one cluster share one UMMA (M = 256); the leader (rank 0) issues it.
+// thread-block clusters
 // ----------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -219,77 +121,46 @@ __device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
   return r;
 }
-// remote arrive (default .release.cta semantics, as CUTLASS' ClusterBarrier::arrive): a cluster-scope release would
-// compile to MEMBAR.ALL.GPU and stall the epilogue warp until all its global stores have drained
-// (profiles/r01_ncu_gemm2_conv.md) — only the TMEM reads, already waited on, need to be ordered before it
+// remote arrive with the default (CTA-scope) release: the only accesses to order before it are this warpgroup's wgmma
+// reads of the stage, already waited on; a cluster-scope release would add a GPU-wide memory fence per K block
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-__device__ __forceinline__ void tma_load_4d_2sm(const void* map, uint32_t bar_cluster_addr, void* dst, int c0, int c1,
-                                                int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, "
-      "%5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar_cluster_addr), "r"(c0), "r"(c1), "r"(c2),
-      "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* dst_smem, uint32_t ncols) {  // one warp in EACH CTA
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2cta() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_ss_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                 uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrives (once all prior MMAs of this thread completed) on the barrier at the same offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_2cta(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
 
 // ----------------------------------------------------------------------------
-// UMMA descriptors (see cute/arch/mma_sm100_desc.hpp for the bit layout)
+// warpgroup MMA plumbing
 // ----------------------------------------------------------------------------
-// K-major operand tile in shared memory written by TMA with SWIZZLE_128B: rows of 64 fp16 (128 B),
-// 8-row swizzle atoms of 1024 B.  start address / LBO / SBO are encoded >>4.
+// before the first wgmma of a batch: orders earlier register / shared-memory accesses of the accumulators and operands
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {  // <= N committed groups still in flight
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int K>
+__device__ __forceinline__ void reg_fence(float (&d)[K]) {
+#pragma unroll
+  for (int i = 0; i < K; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// K-major operand tile in shared memory written by TMA with SWIZZLE_128B: rows of 64 fp16 (128 B), 8-row swizzle atoms
+// of 1024 B (the atom base must be 1024-byte aligned).  Start address and stride byte offset are encoded >> 4; the
+// leading byte offset is unused for swizzled K-major tiles.  Advancing K by 16 elements inside the 128-byte row is
+// +32 B, i.e. +2 on the descriptor.
 __device__ __forceinline__ uint64_t make_desc_k_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);  // [0,14)  start address
-  d |= static_cast<uint64_t>(1) << 16;                 // [16,30) LBO (unused for swizzled K-major)
+  d |= static_cast<uint64_t>(1) << 16;                 // [16,30) LBO (unused)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;         // [32,46) SBO = 8 rows * 128 B
-  d |= static_cast<uint64_t>(1) << 46;                 // [46,48) descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                 // [61,64) SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                 // [62,64) layout: SWIZZLE_128B
   return d;
-}
-// kind::f16 instruction descriptor: fp16 A/B (K-major both), fp32 accumulate, M x N tile.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4)                              // c_format = F32
-         | (0u << 7) | (0u << 10)               // a/b format = F16
-         | (0u << 15) | (0u << 16)              // a/b K-major
-         | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
 }
 
 // ----------------------------------------------------------------------------
 // programmatic dependent launch: a kernel launched with the PDL attribute may start while its predecessor drains;
-// everything before pdl_wait() (barrier init, TMEM alloc, descriptor prefetch) overlaps the predecessor's tail,
-// nothing after it runs until the predecessor grid has completed and its writes are visible.
+// everything before pdl_wait() (barrier init, descriptor prefetch) overlaps the predecessor's tail, nothing after it
+// runs until the predecessor grid has completed and its writes are visible.
 // ----------------------------------------------------------------------------
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -298,32 +169,28 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 // small math helpers
 // ----------------------------------------------------------------------------
 __device__ __forceinline__ float silu_f(float x) { return x / (1.f + __expf(-x)); }
-__device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
-// exact-erf GELU via Abramowitz-Stegun 7.1.26 (|erf error| < 1.5e-7, branch-free: 1 rcp + 1 ex2 + ~12 FMA) — about half
-// the instructions of erff(); the GEGLU GEMM epilogue evaluates it 4C times per token
-__device__ __forceinline__ float gelu_fast_f(float g) {
-  const float z = fabsf(g) * 0.70710678118654752f;
-  const float t = __fdividef(1.f, fmaf(0.3275911f, z, 1.f));
+__device__ __forceinline__ float ex2f(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+// a * gelu(g) with the exact-erf GELU through Abramowitz-Stegun 7.1.26 (|erf error| < 1.5e-7, branch-free:
+// 1 rcp + 1 ex2 + ~10 FMA), rearranged so that no sign handling is left:
+//   g * (1 + erf(g / sqrt2)) = g + |g| * erf(|g| / sqrt2),  erf(z) = 1 - q(t) e^{-z^2},  t = 1 / (1 + p z)
+__device__ __forceinline__ float geglu_f(float a, float g) {
+  const float z = fabsf(g);
+  float t;
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(z, 0.3275911f * 0.70710678118654752f, 1.f)));
   float q = fmaf(1.061405429f, t, -1.453152027f);
   q = fmaf(q, t, 1.421413741f);
   q = fmaf(q, t, -0.284496736f);
   q = fmaf(q, t, 0.254829592f);
   q *= t;
-  float e;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-(z * z) * 1.4426950408889634f));
+  const float e = ex2f(z * z * (-0.5f * 1.4426950408889634f));  // e^{-z^2/2}
   const float erf_abs = fmaf(-q, e, 1.f);
-  return 0.5f * g * (1.f + copysignf(erf_abs, g));
+  return 0.5f * a * fmaf(z, erf_abs, g);
 }
-// packed fp32x2 math (sm_100a FFMA2 / FMUL2 / FADD2): one issue slot for two values
-// register re-balancing between warpgroups (all warps of a warpgroup execute it)
-template <int REGS>
-__device__ __forceinline__ void reg_dealloc() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
-template <int REGS>
-__device__ __forceinline__ void reg_alloc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
-// n / d for a divisor known at plan time: magic = ceil(2^32 / d) (0 encodes d = 1); exact while n * d < 2^32
-__device__ __forceinline__ int fast_div(int n, uint32_t magic) {
-  return magic ? static_cast<int>(__umulhi(static_cast<uint32_t>(n), magic)) : n;
-}
+// fp32 pairs (a float2 in one 64-bit register pair) for the GroupNorm / small-conv kernels
 __device__ __forceinline__ uint64_t pk2(float lo, float hi) {
   uint64_t r;
   asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
@@ -333,46 +200,23 @@ __device__ __forceinline__ void upk2(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
 __device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  upk2(c, c0, c1);
+  return pk2(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 __device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  return pk2(a0 + b0, a1 + b1);
 }
 __device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-// (2 * ah) * gelu(g) for two lanes, ah = HALF the value operand (the 0.5 of GELU is folded into it by the caller).
-// Same Abramowitz-Stegun 7.1.26 erf as gelu_fast_f, rearranged so that no sign handling is left:
-//   g * (1 + erf(g / sqrt2)) = g + |g| * erf(|g| / sqrt2),  erf(z) = 1 - q(t) e^{-z^2},  t = 1 / (1 + p z)
-// ~10 issue slots per value (2 MUFU) instead of ~39 in scalar form — the GEGLU epilogue was instruction bound
-// (profiles/r01_ncu_epilogue_shortk.md).
-__device__ __forceinline__ uint64_t geglu2(uint64_t ah, float g0, float g1) {
-  const uint64_t g = pk2(g0, g1);
-  const uint64_t z = pk2(fabsf(g0), fabsf(g1));  // |g|
-  float d0, d1;
-  upk2(fma2(z, pk2(0.3275911f * 0.70710678118654752f, 0.3275911f * 0.70710678118654752f), pk2(1.f, 1.f)), d0, d1);
-  float t0, t1;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t0) : "f"(d0));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t1) : "f"(d1));
-  const uint64_t t = pk2(t0, t1);
-  uint64_t q = fma2(pk2(-1.061405429f, -1.061405429f), t, pk2(1.453152027f, 1.453152027f));  // -q(t): signs flipped
-  q = fma2(q, t, pk2(-1.421413741f, -1.421413741f));
-  q = fma2(q, t, pk2(0.284496736f, 0.284496736f));
-  q = fma2(q, t, pk2(-0.254829592f, -0.254829592f));
-  q = mul2(q, t);
-  float x0, x1;
-  upk2(mul2(mul2(z, z), pk2(-0.5f * 1.4426950408889634f, -0.5f * 1.4426950408889634f)), x0, x1);  // -z^2/2 * log2(e)
-  float e0, e1;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(x0));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(x1));
-  const uint64_t erf_abs = fma2(q, pk2(e0, e1), pk2(1.f, 1.f));  // 1 - q e
-  return mul2(ah, fma2(z, erf_abs, g));
+  float a0, a1, b0, b1;
+  upk2(a, a0, a1);
+  upk2(b, b0, b1);
+  return pk2(a0 * b0, a1 * b1);
 }
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   __half2 h = __floats2half2_rn(a, b);

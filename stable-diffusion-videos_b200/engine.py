@@ -30,7 +30,7 @@ class Engine:
     def __init__(self, unet_cfg: UNetConfig, vae_cfg: VAEConfig, latent_hw, frames, guidance=True, ctx_tokens=77,
                  max_steps=128, device=None, tiled=False):
         if not torch.cuda.is_available():
-            raise N.SdwError("the native engine needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise N.SdwError("the native engine needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device(device or f"cuda:{torch.cuda.current_device()}")
         self.unet_cfg, self.vae_cfg = unet_cfg, vae_cfg
         self.frames, self.guidance = int(frames), bool(guidance)

@@ -5,7 +5,7 @@ Same method names, argument meaning and error behaviour as the reference for the
 `__call__` (P:192), `generate_inputs` (P:457), `make_clip_frames` (P:481), `walk` (P:556), `embed_text` (P:809),
 `init_noise` (P:822), `from_pretrained(tiled=)` (P:841), plus the duck-typed attributes callers read.
 What differs is WHERE the arithmetic runs: lerp/slerp, the denoise loop (UNet, CFG, scheduler step) and the VAE
-decode + uint8 post-process are native sm_100a kernels behind the C ABI.  There is no diffusers dependency and no
+decode + uint8 post-process are native sm_90a kernels behind the C ABI.  There is no diffusers dependency and no
 CPU fallback: without the CUDA library this class raises.
 """
 import json

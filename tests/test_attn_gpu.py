@@ -1,4 +1,4 @@
-"""GPU parity of the fused tcgen05 attention kernel (sdw_attention) against torch fp32 SDPA.
+"""GPU parity of the fused wgmma attention kernel (sdw_attention) against torch fp32 SDPA.
 Tolerance: P is rounded to fp16 before the PV product and the output is rounded to fp16:
 |err| <= 2^-8 * max|ref| + 1e-3 (calibrated in DESIGN.md §Parity)."""
 import ctypes as C
@@ -66,7 +66,7 @@ def test_flash_attention_peaky_scores():
     (3, 8, 1024, 1024, 40),   # several work items per CTA (persistent loop, Q refill, barrier phases across items)
 ])
 def test_two_tile_kernel_rising_max_and_ragged(B, heads, Nq, Nk, d):
-    """attn_pp_kernel: keys scaled so that the row max keeps rising along the KV loop (lazy rescale engages late too)."""
+    """keys scaled so that the row max keeps rising along the KV loop (the running-max rescale engages on every tile)."""
     from stable_diffusion_videos_b200 import _native as n
 
     g = torch.Generator().manual_seed(5)
@@ -91,7 +91,7 @@ def test_two_tile_kernel_rising_max_and_ragged(B, heads, Nq, Nk, d):
 
 
 def test_one_tile_kernel_still_matches_subprocess():
-    """SDW_ATTN_PP=0 routes head dims <= 64 through attn_fwd_kernel (the A/B switch used by tools/attn_bench.py)"""
+    """a fresh process (first launch of the kernels, no cached attributes) computes the same attention"""
     import os
     import subprocess
     import sys
@@ -110,6 +110,6 @@ def test_one_tile_kernel_still_matches_subprocess():
             "    err=(out.float()-ref).abs().max().item(); assert err <= 2**-8*ref.abs().max().item()+1e-3, (err, B,h,Nq,Nk,d)\n"
             "print('ok')\n")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    env = dict(os.environ, SDW_ATTN_PP="0")
+    env = dict(os.environ)
     r = subprocess.run([sys.executable, "-c", code], env=env, cwd=root, capture_output=True, text=True, timeout=300)
     assert r.returncode == 0 and "ok" in r.stdout, (r.stdout[-500:], r.stderr[-2000:])

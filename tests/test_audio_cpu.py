@@ -116,14 +116,19 @@ def test_package_entry_point_uses_the_restatement_without_librosa(tmp_path):
     assert T.shape == (60,) and abs(T[-1] - 1.0) < 1e-6 and (np.diff(T) > 0).all()
 
 
-def test_cfg5_schedule_fixture(audio):
+def test_cfg5_schedule_fixture(audio, tmp_path):
     """BASELINE configs[4]: T for the reference's own choice.wav with the example's arguments (fps 30, margin 1.0,
-    smooth 0.2) is committed as tests/golden/cfg5_choice_T.npy; where the reference checkout exists the restatement must
-    reproduce it, everywhere it must be a valid schedule (300 frames, in [0, 1], non-decreasing, ends at 1)."""
-    T = np.load(os.path.join(ROOT, "tests", "golden", "cfg5_choice_T.npy"))
+    smooth 0.2) is committed as tests/golden/cfg5_choice_T.npy and must be a valid schedule (300 frames, in [0, 1],
+    non-decreasing, ends at 1); the restatement must reproduce the committed schedule of the wav's first 2 s
+    (tests/golden/choice_2s_i16.npy -> cfg5_choice_2s_T.npy, generator make_cfg5_schedule.py)."""
+    from scipy.io import wavfile
+
+    G = os.path.join(ROOT, "tests", "golden")
+    T = np.load(os.path.join(G, "cfg5_choice_T.npy"))
     assert T.shape == (300,) and T.dtype == np.float64
     assert T.min() >= 0.0 and abs(T[-1] - 1.0) < 1e-12 and np.all(np.diff(T) >= 0)
-    wav = "/root/reference/tests/samples/choice.wav"
-    if os.path.exists(wav):
-        again = audio.get_timesteps_arr(wav, offset=0, duration=10, fps=30, margin=1.0, smooth=0.2)
-        assert np.allclose(again, T, atol=1e-9)
+    wav = tmp_path / "choice_2s.wav"
+    wavfile.write(wav, 22050, np.load(os.path.join(G, "choice_2s_i16.npy")))
+    want = np.load(os.path.join(G, "cfg5_choice_2s_T.npy"))
+    again = audio.get_timesteps_arr(str(wav), offset=0, duration=2, fps=30, margin=1.0, smooth=0.2)
+    assert want.shape == (60,) and np.allclose(again, want, atol=1e-9)

@@ -117,8 +117,9 @@ def test_launch_plans_validate_without_a_gpu():
 @pytest.mark.parametrize("toggle", ["SDW_GEMM_EW=2", "SDW_GEMM_EW=4", "SDW_EPI_TMA=0", "SDW_EPI_TMA=2", "SDW_GEMM_TR=0",
                                     "SDW_NO_FLASH=1"])
 def test_launch_plans_validate_under_every_opt_in_switch(toggle):
-    """the kernel A/B switches (8-warp epilogue everywhere, classic epilogue, per-tap conv loads, ...) must
-    plan the full SD-1.4 engine too: shared-memory budgets, tensor-map alignment, stage counts (plan-only, no GPU)."""
+    """the full SD-1.4 engine must plan under environment switches too — the unfused-attention path, and switch names of
+    earlier builds, which must not disturb planning: shared-memory budgets, tensor-map alignment, stage counts (plan-only,
+    no GPU)."""
     import os
     import subprocess
     import sys

@@ -32,7 +32,8 @@ def bench(B, heads, Nq, Nk, d, iters=10):
     ms = e0.elapsed_time(e1) / iters
     flop = 4.0 * B * heads * Nq * Nk * d
     pairs = B * heads * Nq * Nk
-    mufu_floor_us = pairs / (16 * 148 * 1.9e9) * 1e6
+    n_sm = torch.cuda.get_device_properties(0).multi_processor_count
+    mufu_floor_us = pairs / (16 * n_sm * 1.98e9) * 1e6  # one ex2 per score, 16 / clk / SM at the 1980 MHz boost clock
     return ms, flop / ms / 1e9, mufu_floor_us
 
 

@@ -1,4 +1,4 @@
-"""one attention shape, a few launches — target for `ncu --set full -k regex:attn_fwd`."""
+"""one attention shape, a few launches — target for `ncu --set full -k regex:attn_kernel`."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
-"""Micro-benchmark of the tcgen05 implicit-GEMM kernel on representative SD-1.4 shapes (CUDA events, warm).
-Prints TFLOP/s per shape; used to steer kernel work and to produce profiles/*_gemm_shapes.txt."""
+"""Micro-benchmark of the wgmma implicit-GEMM kernel on representative SD-1.4 shapes (CUDA events, warm).
+Prints TFLOP/s per shape and plan variant."""
 import os
 import sys
 
@@ -64,6 +64,10 @@ if __name__ == "__main__":
                             (256, 1, 1), (256, 1, 2), (160, 2, 1), (160, 2, 2))
             for bn, nsub, tr in variants:
                 for epi in (True,):
-                    ms, tf = bench(B, H, W, C, N, conv, bn=bn, ver=ver, epi=epi, nsub=nsub, tr=tr)
+                    try:
+                        ms, tf = bench(B, H, W, C, N, conv, bn=bn, ver=ver, epi=epi, nsub=nsub, tr=tr)
+                    except n.SdwError as e:  # a variant the planner refuses for this shape
+                        print(f"{name:36s} B={B:3d} v{ver} bn={bn or 'auto':>4} nsub={nsub} tr={tr} refused: {e}", flush=True)
+                        continue
                     print(f"{name:36s} B={B:3d} v{ver} bn={bn or 'auto':>4} nsub={nsub} tr={tr} "
                           f"epi={'bias+res' if epi else 'none':8s} {ms*1e3:9.1f} us {tf:8.1f} TFLOP/s", flush=True)
