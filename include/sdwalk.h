@@ -218,6 +218,32 @@ int sdw_groupnorm(const void* x, int64_t ldx, int B, int64_t P, int C, int G, co
 int sdw_layernorm(const void* x, int64_t ldx, int64_t rows, int C, const float* gamma, const float* beta, float eps,
                   void* y, int64_t ldy, void* stream);
 
+/* the remaining layers of the sampler, one entry point per kernel (tests / tooling); fp16 tensors are NHWC.
+ *   softmax_rows   : in place over `rows` rows of n fp16 scores at pitch ld (the unfused attention's middle step)
+ *   conv_in_small  : 3x3 pad 1 conv, Cin (= 4) -> N <= 512 channels; w OIHW fp16 [N][Cin][3][3], bias fp32 [N] or null
+ *   conv_out_small : 3x3 pad 1 conv, C -> nout (3 or 4) channels; out_f32 fp32 [B][H][W][nout] and/or
+ *                    out_u8 uint8 [B][H][W][nout] = round(clamp(v/2 + 0.5, 0, 1) * 255), either may be null
+ *   vae_in         : z = W (x * inv_scale) + b, x fp32 NCHW [F][C][H][W] (C <= 8), W fp16 [C][C], z fp16 [F][H][W][C]
+ *   timestep_embed : out fp32 [n][dim] = cat[cos(t f), sin(t f)], rounded to fp16 values when round_f16
+ *   linear_f32     : out[m][n] = act_out(bias[n] + sum_k act_in(in[m][k]) W[n][k]), fp32 in / out, W fp16 [N][K];
+ *                    act = SiLU when silu_in / silu_out
+ *   wrap_pad       : y [B][H+2pad][W+2pad] dense pixels of pix_bytes = circularly padded copy of x (pixel pitch ld_bytes)
+ *   crop_interior  : out (pixel pitch ldo_bytes) = interior of the [B][H+2crop][W+2crop] image yp, plus the fp16
+ *                    residual resid_f16 (pixel pitch ldr elements) when non-null */
+int sdw_softmax_rows(void* s, int64_t ld, int64_t rows, int n, void* stream);
+int sdw_conv_in_small(const void* x, int64_t ldx, int B, int H, int W, int Cin, const void* w, const float* bias, int N,
+                      void* y, int64_t ldy, void* stream);
+int sdw_conv_out_small(const void* x, int64_t ldx, int B, int H, int W, int C, const void* w, const float* bias, int nout,
+                       float* out_f32, uint8_t* out_u8, void* stream);
+int sdw_vae_in(const float* x, float inv_scale, const void* w, const float* bias, int F, int C, int H, int W, void* z,
+               void* stream);
+int sdw_timestep_embed(const float* t, int n, int dim, int round_f16, float* out, void* stream);
+int sdw_linear_f32(const float* in, int64_t ldi, const void* w, const float* bias, int M, int N, int K, int silu_in,
+                   int silu_out, float* out, int64_t ldo, void* stream);
+int sdw_wrap_pad(const void* x, int64_t ld_bytes, int B, int H, int W, int pix_bytes, int pad, void* y, void* stream);
+int sdw_crop_interior(const void* yp, int B, int H, int W, int pix_bytes, int crop, const void* resid_f16, int64_t ldr,
+                      void* out, int64_t ldo_bytes, void* stream);
+
 /* attention planner introspection, host only: out = {kernel variant, query tiles per CTA, grid x, y, z} */
 int sdw_debug_attention_plan(int B, int Nq, int Nk, int heads, int d, int32_t out[5]);
 

@@ -121,6 +121,47 @@ int sdw_layernorm(const void* x, int64_t ldx, int64_t rows, int C, const float* 
                    static_cast<cudaStream_t>(stream));
 }
 
+int sdw_softmax_rows(void* s, int64_t ld, int64_t rows, int n, void* stream) {
+  return softmax_rows(static_cast<__half*>(s), ld, rows, n, static_cast<cudaStream_t>(stream));
+}
+
+int sdw_conv_in_small(const void* x, int64_t ldx, int B, int H, int W, int Cin, const void* w, const float* bias, int N,
+                      void* y, int64_t ldy, void* stream) {
+  return conv_in_small(static_cast<const __half*>(x), ldx, B, H, W, Cin, static_cast<const __half*>(w), bias, N,
+                       static_cast<__half*>(y), ldy, static_cast<cudaStream_t>(stream));
+}
+
+int sdw_conv_out_small(const void* x, int64_t ldx, int B, int H, int W, int C, const void* w, const float* bias, int nout,
+                       float* out_f32, uint8_t* out_u8, void* stream) {
+  return conv_out_small(static_cast<const __half*>(x), ldx, B, H, W, C, static_cast<const __half*>(w), bias, nout, out_f32,
+                        out_u8, static_cast<cudaStream_t>(stream));
+}
+
+int sdw_vae_in(const float* x, float inv_scale, const void* w, const float* bias, int F, int C, int H, int W, void* z,
+               void* stream) {
+  return vae_in(x, inv_scale, static_cast<const __half*>(w), bias, F, C, H, W, static_cast<__half*>(z),
+                static_cast<cudaStream_t>(stream));
+}
+
+int sdw_timestep_embed(const float* t, int n, int dim, int round_f16, float* out, void* stream) {
+  return timestep_embed(t, n, dim, round_f16, out, static_cast<cudaStream_t>(stream));
+}
+
+int sdw_linear_f32(const float* in, int64_t ldi, const void* w, const float* bias, int M, int N, int K, int silu_in,
+                   int silu_out, float* out, int64_t ldo, void* stream) {
+  return linear_f32(in, ldi, static_cast<const __half*>(w), bias, M, N, K, silu_in, silu_out, out, ldo,
+                    static_cast<cudaStream_t>(stream));
+}
+
+int sdw_wrap_pad(const void* x, int64_t ld_bytes, int B, int H, int W, int pix_bytes, int pad, void* y, void* stream) {
+  return wrap_pad(x, ld_bytes, B, H, W, pix_bytes, pad, y, static_cast<cudaStream_t>(stream));
+}
+
+int sdw_crop_interior(const void* yp, int B, int H, int W, int pix_bytes, int crop, const void* resid_f16, int64_t ldr,
+                      void* out, int64_t ldo_bytes, void* stream) {
+  return crop_interior(yp, B, H, W, pix_bytes, crop, resid_f16, ldr, out, ldo_bytes, static_cast<cudaStream_t>(stream));
+}
+
 int sdw_debug_attention_plan(int B, int Nq, int Nk, int heads, int d, int32_t out[5]) {
   SDW_REQUIRE(out != nullptr, "null");
   AttnDesc a;

@@ -85,3 +85,63 @@ def test_layernorm_strided_rows(Cc):
     assert (ybuf[:, :64] == 0).all() and (ybuf[:, 64 + Cc:] == 0).all()
     ref = Fn.layer_norm(x.float(), (Cc,), gamma, beta, 1e-5)
     assert (y.float() - ref).abs().max().item() <= 2 ** -9 * ref.abs().max().item() + 1e-3
+
+
+def _gn_ref64(x, G, gamma, beta, eps, silu):
+    ref = Fn.group_norm(x.double().permute(0, 3, 1, 2), G, gamma.double(), beta.double(), eps)
+    return (Fn.silu(ref) if silu else ref).permute(0, 2, 3, 1)
+
+
+@pytest.mark.parametrize("Cc", [320, 640])
+@pytest.mark.parametrize("offset", [0, 64, 256, 512])
+def test_groupnorm_large_mean(offset, Cc):
+    """groups whose mean is large against their spread (std 1): the statistics must not cancel"""
+    n = _native()
+    B, H, W, G = 2, 32, 32, 32
+    x = _rand(B, H, W, Cc, seed=12, shift=float(offset))
+    gamma = _rand(Cc, seed=13).float() * 0.2 + 1.0
+    beta = _rand(Cc, seed=14).float() * 0.1
+    y = torch.full_like(x, float("nan"))
+    n.groupnorm(x, B, H * W, Cc, G, gamma, beta, 1e-5, 0, y)
+    torch.cuda.synchronize()
+    ref = _gn_ref64(x, G, gamma, beta, 1e-5, 0)
+    err = (y.double() - ref).abs().max().item()
+    assert err <= 2 ** -9 * ref.abs().max().item() + 1e-3, err
+
+
+@pytest.mark.parametrize("B,H,W,Cc,G,silu", [
+    (2, 16, 16, 320, 8, 1), (2, 16, 16, 320, 16, 0), (2, 16, 16, 640, 64, 1),
+    (2, 8, 8, 64, 64, 0),     # one channel per group
+    (2, 8, 8, 32, 8, 1),      # the tiny test configuration's first level
+    (3, 1, 1, 320, 32, 1),    # P < 16: a single statistics chunk
+    (2, 3, 3, 640, 32, 0),
+    (2, 1, 1, 64, 64, 0),     # one value per group: variance 0
+])
+def test_groupnorm_group_counts_and_tiny_images(B, H, W, Cc, G, silu):
+    n = _native()
+    x = _rand(B, H, W, Cc, seed=15, scale=1.5, shift=0.3)
+    gamma = _rand(Cc, seed=16).float() * 0.2 + 1.0
+    beta = _rand(Cc, seed=17).float() * 0.1
+    y = torch.full_like(x, float("nan"))
+    n.groupnorm(x, B, H * W, Cc, G, gamma, beta, 1e-5, silu, y)
+    torch.cuda.synchronize()
+    ref = _gn_ref64(x, G, gamma, beta, 1e-5, silu)
+    assert torch.isfinite(y.float()).all()
+    assert (y.double() - ref).abs().max().item() <= 2 ** -9 * ref.abs().max().item() + 1e-3
+
+
+@pytest.mark.parametrize("Cc", [320, 768])
+@pytest.mark.parametrize("offset", [0, 64, 256, 512])
+def test_layernorm_large_mean(offset, Cc):
+    """the same offset sweep for LayerNorm (two-pass statistics)"""
+    n = _native()
+    rows = 1000
+    x = _rand(rows, Cc, seed=18, shift=float(offset))
+    gamma = _rand(Cc, seed=19).float() * 0.2 + 1.0
+    beta = _rand(Cc, seed=20).float() * 0.1
+    y = torch.full_like(x, float("nan"))
+    n.layernorm(x, rows, Cc, gamma, beta, 1e-5, y)
+    torch.cuda.synchronize()
+    ref = Fn.layer_norm(x.double(), (Cc,), gamma.double(), beta.double(), 1e-5)
+    err = (y.double() - ref).abs().max().item()
+    assert err <= 2 ** -9 * ref.abs().max().item() + 1e-3, err
