@@ -3,16 +3,24 @@
 //
 //   O[b, q, h*d:(h+1)*d] = softmax(Q_h K_h^T * d^-1/2) V_h          per (batch b, head h), fp16 in / fp16 out
 //
-// Nothing but Q, K, V^T tiles and the O tile touches HBM.  One CTA = one 128-query tile of one (b, h):
-//   warp 8    : TMA producer — the Q tile once, then K and V^T tiles of BKV keys into a ring of ST stages.  The head
-//               dimension is loaded in 64-column boxes whose columns beyond d are zero-filled by TMA, and V^T rows
-//               beyond d likewise, so padding needs no code.
-//   warps 0-7 : two consumer warpgroups, 64 query rows each.  Per KV tile: S = Q K^T (wgmma m64nBKVk16, operands in
-//               shared memory, fp32 scores in registers), online softmax in registers (a query row lives in the four
-//               lanes of a quad), P rounded to fp16 and fed straight from registers as the A operand of
-//               O += P V (wgmma m64nDVPk16, register-A form), then the stage is released.  The two warpgroups
-//               interleave on the SM: one's exponentials overlap the other's MMAs.
-// Ordering is carried by mbarriers only.
+// Nothing but Q, K, V^T tiles and the O tile touches HBM.  One CTA = one 128-query tile of one (b, h), 384 threads:
+//   warpgroup 2 (warps 8-11): producer, its registers handed to the consumers (setmaxnreg).  One thread TMA-loads the Q
+//               tile once, then K and V^T tiles of BKV keys into a ring of ST stages.  The head dimension is loaded
+//               in 64-column boxes whose columns beyond d are zero-filled by TMA, and V^T rows beyond d likewise, so
+//               padding needs no code: the QK^T k-step count is DVP / 16 for every d of a variant.
+//   warpgroups 0, 1: consumers, 64 query rows each.  S = Q K^T is wgmma m64nBKVk16 with both operands in shared
+//               memory and fp32 scores in registers; the online softmax runs in registers (a query row lives in the
+//               four lanes of a quad); P is rounded to fp16 and fed straight from registers as the A operand of
+//               O += P V (wgmma m64nDVPk16, register-A form).
+// Two overlaps keep MUFU (the exponentials) and the tensor cores busy at the same time:
+//   - within a warpgroup, KV tile j's scores are issued together with tile j-1's PV product, and the softmax of tile j
+//     runs while that PV product is still in flight (wgmma_wait<1>); O is rescaled only after it has landed;
+//   - between the warpgroups (ping-pong), named barriers order the MMA issues: a warpgroup issues its two GEMMs only
+//     after the other has issued its own, so one warpgroup's exponentials run under the other's MMAs.  Every
+//     warpgroup passes every barrier whatever its rows, and the order does not change any arithmetic: the result is
+//     the same bits on every run.
+// No accumulator register is written between a wgmma issue and its wait (the C7515 serialisation of ptxas).  Stage
+// ordering is carried by mbarriers; a stage is released once the PV product that reads its V^T has completed.
 #include "sdw_internal.h"
 #include "sdw_ptx.cuh"
 
@@ -22,14 +30,17 @@
 
 namespace sdw {
 
-static constexpr int ATT_THREADS = 288;  // two consumer warpgroups + one producer warp
+static constexpr int ATT_THREADS = 384;  // two consumer warpgroups + one producer warpgroup
 static constexpr int ATT_BQ = 128;
-static constexpr int ATT_ST = 3;
+static constexpr int ATT_ST = 4;
+// launched at <= 168 registers per thread (64K / 384); the producer gives 128 x 144 of them to the consumers
+static constexpr int ATT_PRODUCER_REGS = 24;
+static constexpr int ATT_CONSUMER_REGS = 240;
+static constexpr int ATT_BAR_PINGPONG = 1;  // named barriers 1 and 2: "consumer warpgroup 0 / 1 may issue its MMAs"
 
 struct alignas(64) AttnKParams {
   CUtensorMap mapQ, mapK, mapV;
   int Nq, Nk, d, heads;
-  int dk_steps;          // ceil(d / 16)
   float scale_log2e;     // d^-1/2 * log2(e)
   __half* out;
   int64_t out_ld;
@@ -39,15 +50,89 @@ struct alignas(64) AttnKParams {
 // DKC 64-column chunks of the head dimension for Q and K; DVP = head dimension padded for the PV tile width
 template <int DKC, int DVP, int BKV>
 struct AttnCfg {
+  static constexpr int KSTEPS = DVP / 16;  // QK^T k-steps of 16 head-dim columns
   static constexpr int Q_BYTES = DKC * ATT_BQ * 128;
   static constexpr int K_CHUNK = BKV * 128;
   static constexpr int K_STAGE = DKC * K_CHUNK;
   static constexpr int V_BOX = DVP * 128;  // one 64-key box of V^T rows
   static constexpr int V_STAGE = (BKV / 64) * V_BOX;
   static constexpr int SMEM = 1024 /*align*/ + 1024 /*barriers*/ + Q_BYTES + ATT_ST * (K_STAGE + V_STAGE);
+  static_assert(KSTEPS <= 4 * DKC, "k-steps beyond the loaded head-dim chunks");
   static_assert(V_BOX % 1024 == 0 && K_CHUNK % 1024 == 0, "swizzle atoms must stay 1024-byte aligned");
   static_assert(SMEM <= 227 * 1024, "shared memory");
 };
+
+// S = Q K^T of one KV stage for the warpgroup's 64 rows (one wgmma group)
+template <int DKC, int DVP, int BKV>
+__device__ __forceinline__ void attn_issue_s(float (&s)[BKV / 2], uint32_t q_base, uint32_t k_base) {
+  using Cfg = AttnCfg<DKC, DVP, BKV>;
+#pragma unroll
+  for (int kk = 0; kk < Cfg::KSTEPS; ++kk) {
+    const uint64_t dq = make_desc_k_sw128(q_base + (kk / 4) * ATT_BQ * 128);
+    const uint64_t dk = make_desc_k_sw128(k_base + (kk / 4) * Cfg::K_CHUNK);
+    Wgmma<BKV>::ss(s, dq + 2 * (kk % 4), dk + 2 * (kk % 4), kk > 0 ? 1u : 0u);
+  }
+  wgmma_commit();
+}
+
+// O += P V of one KV stage (one wgmma group); P as fp16 A fragments in registers
+template <int DKC, int DVP, int BKV>
+__device__ __forceinline__ void attn_issue_pv(float (&o)[DVP / 2], const uint32_t (&pa)[BKV / 16][4], uint32_t v_base) {
+  using Cfg = AttnCfg<DKC, DVP, BKV>;
+#pragma unroll
+  for (int kk = 0; kk < BKV / 16; ++kk)
+    Wgmma<DVP>::rs(o, pa[kk], make_desc_k_sw128(v_base + (kk / 4) * Cfg::V_BOX) + 2 * (kk % 4), 1u);
+  wgmma_commit();
+}
+
+// One KV tile's online-softmax step on the warpgroup's fp32 scores (row r in s[4jb + 0..1], row r + 8 in
+// s[4jb + 2..3], columns 8jb + 2(lane % 4) + {0, 1}).  The running max m is kept in raw score units, so each
+// probability is one FFMA and one ex2: 2^(s c - m c) with c = d^-1/2 log2(e).  s is replaced in place by these
+// probabilities, l is updated, and corr receives the factor O must be rescaled by.  MASK: keys at columns >= valid
+// get probability 0; only the last KV tile can be ragged.
+template <int BKV, bool MASK>
+__device__ __forceinline__ void attn_softmax(float (&s)[BKV / 2], int valid, float c, float (&m)[2], float (&l)[2],
+                                             float (&corr)[2]) {
+  const int q2 = 2 * (threadIdx.x & 3);
+  // four partial maxima and two partial sums per row: short dependency chains, so the one warp of each warpgroup on
+  // a scheduler is not left waiting on FMNMX / FADD latency
+  float mx4[2][4];
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+    for (int i = 0; i < 4; ++i) mx4[hh][i] = m[hh];
+#pragma unroll
+  for (int jb = 0; jb < BKV / 8; ++jb)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float& x = s[4 * jb + 2 * hh + e];
+        if (MASK && 8 * jb + q2 + e >= valid) x = -INFINITY;
+        mx4[hh][2 * (jb & 1) + e] = fmaxf(mx4[hh][2 * (jb & 1) + e], x);
+      }
+  float mx[2], mc[2], sum[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    mx[hh] = fmaxf(fmaxf(mx4[hh][0], mx4[hh][1]), fmaxf(mx4[hh][2], mx4[hh][3]));
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+    mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+    corr[hh] = ex2f((m[hh] - mx[hh]) * c);  // the first tile: 2^-inf = 0 (every tile holds a key, so mx is finite)
+    m[hh] = mx[hh];
+    mc[hh] = mx[hh] * c;
+  }
+#pragma unroll
+  for (int jb = 0; jb < BKV / 8; ++jb)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      float* x = &s[4 * jb + 2 * hh];
+      x[0] = ex2f(fmaf(x[0], c, -mc[hh]));
+      x[1] = ex2f(fmaf(x[1], c, -mc[hh]));
+      sum[hh][jb & 1] += x[0] + x[1];
+    }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) l[hh] = l[hh] * corr[hh] + (sum[hh][0] + sum[hh][1]);
+}
 
 template <int DKC, int DVP, int BKV>
 __global__ void __launch_bounds__(ATT_THREADS, 1) attn_kernel(const __grid_constant__ AttnKParams p) {
@@ -80,9 +165,10 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_kernel(const __grid_const
   pdl_wait();
   pdl_launch_dependents();
 
-  if (warp == 8) {
+  if (warp >= 8) {
     // =========================== TMA producer ===============================
-    if (lane == 0) {
+    setmaxnreg_dec<ATT_PRODUCER_REGS>();
+    if (warp == 8 && lane == 0) {
       mbar_expect_tx(q_full, Cfg::Q_BYTES);
 #pragma unroll
       for (int c = 0; c < DKC; ++c) tma_load_4d(&p.mapQ, q_full, sQ + c * ATT_BQ * 128, 64 * c, qt * ATT_BQ, h, b);
@@ -107,72 +193,74 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_kernel(const __grid_const
   }
 
   // =========================== consumers ======================================
+  setmaxnreg_inc<ATT_CONSUMER_REGS>();
   const int wg = warp >> 2;
-  const int q2 = 2 * (lane & 3);
+  const uint32_t bar_mine = ATT_BAR_PINGPONG + wg, bar_other = ATT_BAR_PINGPONG + (wg ^ 1);
+  const float c = p.scale_log2e;
+  const int last_valid = p.Nk - (nkv - 1) * BKV;  // keys in the last KV tile
   float o[DVP / 2];
 #pragma unroll
   for (int i = 0; i < DVP / 2; ++i) o[i] = 0.f;
-  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, corr[2];
+  float s[BKV / 2];          // scores of the newest KV tile, then its probabilities
+  uint32_t pa[BKV / 16][4];  // probabilities of the previous KV tile as fp16 A fragments, read by its PV product
   const uint32_t q_base = smem_u32(sQ) + wg * (64 * 128);
-  mbar_wait(q_full, 0);
 
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int j = 0; j < nkv; ++j) {
-    mbar_wait(&full_bar[stage], phase);
-    // ---- S = Q K^T ----
-    float s[BKV / 2];
-    wgmma_fence();
-    const uint32_t k_base = smem_u32(sK + stage * Cfg::K_STAGE);
-#pragma unroll
-    for (int c = 0; c < DKC; ++c) {
-      const uint64_t dq = make_desc_k_sw128(q_base + c * ATT_BQ * 128);
-      const uint64_t dk = make_desc_k_sw128(k_base + c * Cfg::K_CHUNK);
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        const int kk = 4 * c + ks;
-        if (kk < p.dk_steps) Wgmma<BKV>::ss(s, dq + 2 * ks, dk + 2 * ks, kk > 0 ? 1u : 0u);
-      }
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(s);
-
-    // ---- online softmax (base 2), keys beyond Nk masked ----
-    const int valid = p.Nk - j * BKV;
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int jb = 0; jb < BKV / 8; ++jb)
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float& x = s[4 * jb + 2 * hh + e];
-          x = (8 * jb + q2 + e < valid) ? x * p.scale_log2e : -INFINITY;
-          mx[hh] = fmaxf(mx[hh], x);
-        }
-    float corr[2], sum[2] = {0.f, 0.f};
-#pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
-      mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
-      const float mn = fmaxf(m[hh], mx[hh]);
-      corr[hh] = ex2f(m[hh] - mn);
-      m[hh] = mn;
-    }
-    uint32_t pa[BKV / 16][4];
+  // A fragment of k16 block kb: {row r, k 2q..}, {row r+8, k 2q..}, {row r, k 8+2q..}, {row r+8, k 8+2q..}
+  auto pack_p = [&]() {
 #pragma unroll
     for (int jb = 0; jb < BKV / 8; ++jb) {
-      float e0 = ex2f(s[4 * jb + 0] - m[0]), e1 = ex2f(s[4 * jb + 1] - m[0]);
-      float e2 = ex2f(s[4 * jb + 2] - m[1]), e3 = ex2f(s[4 * jb + 3] - m[1]);
-      sum[0] += e0 + e1;
-      sum[1] += e2 + e3;
-      // A fragment of k16 block jb / 2: {row r, k 2q..}, {row r+8, k 2q..}, {row r, k 8+2q..}, {row r+8, k 8+2q..}
-      pa[jb / 2][2 * (jb & 1) + 0] = pack_h2(e0, e1);
-      pa[jb / 2][2 * (jb & 1) + 1] = pack_h2(e2, e3);
+      pa[jb / 2][2 * (jb & 1) + 0] = pack_h2(s[4 * jb + 0], s[4 * jb + 1]);
+      pa[jb / 2][2 * (jb & 1) + 1] = pack_h2(s[4 * jb + 2], s[4 * jb + 3]);
     }
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh) l[hh] = l[hh] * corr[hh] + sum[hh];
+    for (int kb = 0; kb < BKV / 16; ++kb)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(pa[kb][i])::"memory");
+  };
+  auto softmax = [&](int j) {
+    if (j == nkv - 1 && last_valid < BKV)
+      attn_softmax<BKV, true>(s, last_valid, c, m, l, corr);
+    else
+      attn_softmax<BKV, false>(s, BKV, c, m, l, corr);
+  };
+
+  // warpgroup 0 issues first; afterwards each warpgroup waits for the other's issue before its own (bar_mine) and
+  // lets the other go once its own GEMMs are issued (bar_other).  Per CTA both warpgroups issue nkv + 1 times.
+  if (wg == 1) named_bar_arrive(ATT_BAR_PINGPONG, 256);
+  mbar_wait(q_full, 0);
+
+  // ---- prologue: S of KV tile 0 ----
+  mbar_wait(&full_bar[0], 0);
+  named_bar_sync(bar_mine, 256);
+  wgmma_fence();
+  attn_issue_s<DKC, DVP, BKV>(s, q_base, smem_u32(sK));
+  named_bar_arrive(bar_other, 256);
+  wgmma_wait<0>();
+  reg_fence(s);
+  softmax(0);
+  pack_p();
+
+  int stage = 0;  // stage of KV tile j - 1
+  uint32_t phase = 0;
+  for (int j = 1; j < nkv; ++j) {
+    const int next = stage + 1 == ATT_ST ? 0 : stage + 1;
+    const uint32_t next_phase = next == 0 ? phase ^ 1 : phase;
+    mbar_wait(&full_bar[next], next_phase);
+    // ---- issue S_j = Q K_j^T and O += P_{j-1} V_{j-1} ----
+    named_bar_sync(bar_mine, 256);
+    reg_fence(o);
+    wgmma_fence();
+    attn_issue_s<DKC, DVP, BKV>(s, q_base, smem_u32(sK + next * Cfg::K_STAGE));
+    attn_issue_pv<DKC, DVP, BKV>(o, pa, smem_u32(sV + stage * Cfg::V_STAGE));
+    named_bar_arrive(bar_other, 256);
+    // ---- softmax of tile j under the PV product of tile j - 1 ----
+    wgmma_wait<1>();
+    reg_fence(s);
+    softmax(j);
+    wgmma_wait<0>();
+    reg_fence(o);
+    if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
 #pragma unroll
     for (int jb = 0; jb < DVP / 8; ++jb) {
       o[4 * jb + 0] *= corr[0];
@@ -180,26 +268,23 @@ __global__ void __launch_bounds__(ATT_THREADS, 1) attn_kernel(const __grid_const
       o[4 * jb + 2] *= corr[1];
       o[4 * jb + 3] *= corr[1];
     }
-
-    // ---- O += P V ----
-    wgmma_fence();
-    const uint32_t v_base = smem_u32(sV + stage * Cfg::V_STAGE);
-#pragma unroll
-    for (int kk = 0; kk < BKV / 16; ++kk) {
-      const uint64_t dv = make_desc_k_sw128(v_base + (kk / 4) * Cfg::V_BOX);
-      Wgmma<DVP>::rs(o, pa[kk], dv + 2 * (kk % 4), 1u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    reg_fence(o);
-    if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
-    if (++stage == ATT_ST) {
-      stage = 0;
-      phase ^= 1;
-    }
+    pack_p();
+    stage = next;
+    phase = next_phase;
   }
 
+  // ---- drain: O += P V of the last tile ----
+  named_bar_sync(bar_mine, 256);
+  reg_fence(o);
+  wgmma_fence();
+  attn_issue_pv<DKC, DVP, BKV>(o, pa, smem_u32(sV + stage * Cfg::V_STAGE));
+  if (wg == 0) named_bar_arrive(bar_other, 256);  // warpgroup 1 issues last: nobody waits for its arrival
+  wgmma_wait<0>();
+  reg_fence(o);
+  if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[stage]);
+
   // ---- normalise and store ----
+  const int q2 = 2 * (lane & 3);
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     l[hh] += __shfl_xor_sync(0xffffffffu, l[hh], 1);
@@ -268,7 +353,6 @@ int plan_attention(const AttnDesc& a, AttnLaunch* L) {
   const int dvp = dvp_tab[I->variant];
   AttnKParams& p = I->p;
   p.Nq = a.Nq; p.Nk = a.Nk; p.d = a.d; p.heads = a.heads;
-  p.dk_steps = (a.d + 15) / 16;
   p.scale_log2e = (1.f / std::sqrt(static_cast<float>(a.d))) * 1.4426950408889634f;
   p.out = a.out; p.out_ld = a.out_ld;
   p.vec2 = (a.out_ld % 2 == 0) && (reinterpret_cast<uintptr_t>(a.out) & 3) == 0;

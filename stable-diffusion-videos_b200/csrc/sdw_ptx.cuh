@@ -61,6 +61,31 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // ----------------------------------------------------------------------------
+// named barriers (ids 1..15; id 0 is __syncthreads) over `count` threads, a multiple of 32.  bar.arrive counts the
+// calling warp towards the barrier without waiting; bar.sync counts it and waits until `count` threads have arrived.
+// ----------------------------------------------------------------------------
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// ----------------------------------------------------------------------------
+// per-warpgroup register budget (all 128 threads of the warpgroup execute it): a warp-specialised kernel launched at
+// R registers per thread moves registers from its producer warpgroup (dec) to its consumer warpgroups (inc).  N is a
+// multiple of 8 in [24, 256]; inc waits until the registers are free.
+// ----------------------------------------------------------------------------
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+
+// ----------------------------------------------------------------------------
 // TMA tiled loads (global -> shared, completion on an mbarrier)
 // ----------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const void* map) {
