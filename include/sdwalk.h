@@ -184,12 +184,12 @@ typedef struct sdw_gemm_desc {
   int64_t ldc;
   int64_t o_sW, o_sH, o_sB;
   int32_t mode;              /* 0 plain, 1 GEGLU, 2 QKV with V^T scatter */
-  int32_t act;
+  int32_t act;               /* 0 none, 1 SiLU, 2 LeakyReLU(0.2) */
   float alpha;
   int32_t vt_col0, vt_d, vt_heads, vt_ntok;
   void* vt;
   int64_t vt_ld;
-  int32_t bn;                /* BLOCK_N: 0 auto, 64/128/160/256 */
+  int32_t bn;                /* BLOCK_N: 0 auto, 64/128/160/256 (192: CTA pairs only; 32: single CTAs only, never automatic) */
   int32_t ver;               /* 0 auto, 1: single CTAs, 2: CTA pairs (clusters of two sharing each weight tile by multicast) */
   int32_t nsub;              /* 0 auto, 1 / 2: accumulators per activation tile (2: CTA pairs, BLOCK_N 160) */
   int32_t ew;                /* 0 auto or 2: epilogue warps per 32 accumulator rows (the kernel has one epilogue width) */
@@ -278,6 +278,44 @@ int sdw_clip_missing_params(const sdw_clip* e, const char** first_missing);
 /* ids: device int32 [B][max_positions] (token ids, already padded / truncated by the tokenizer);
  * out: device fp16 [B][max_positions][hidden] = last_hidden_state after the final LayerNorm */
 int sdw_clip_forward(sdw_clip* e, const int32_t* ids, int B, void* out_f16, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Real-ESRGAN x4 upsampler: replaces `self.upsampler(image)` of make_clip_frames(upsample=True)
+ * (stable_diffusion_pipeline.py:513-516, 550-553; upsampling.py RealESRGANModel, whose network is basicsr's RRDBNet).
+ * Parameter names are RRDBNet state-dict keys ("conv_first.weight", "body.{i}.rdb{1,2,3}.conv{1..5}.weight", ...,
+ * "conv_last.bias"), handed over as fp16 in their own layout (OIHW / vectors).  x4 only, num_feat 64, num_grow_ch 32;
+ * num_block is free (23: RealESRGAN_x4plus, 6: the anime model).  Life cycle as the CLIP tower:
+ * create -> arena_bytes -> bind(arena: caller-owned device memory, 256-byte aligned) -> load_param x N -> run x M.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct sdw_upsampler sdw_upsampler;
+typedef struct sdw_upsampler_config {
+  int32_t num_feat, num_block, num_grow_ch;
+  int32_t in_h, in_w;   /* input frame size; the output is 4 in_h x 4 in_w */
+  int32_t frames;       /* frames per run call */
+} sdw_upsampler_config;
+int sdw_upsampler_create(const sdw_upsampler_config* cfg, sdw_upsampler** out);
+void sdw_upsampler_destroy(sdw_upsampler* e);
+int sdw_upsampler_arena_bytes(const sdw_upsampler* e, uint64_t* bytes);
+int sdw_upsampler_bind(sdw_upsampler* e, void* arena, uint64_t bytes);
+int sdw_upsampler_num_params(const sdw_upsampler* e);
+int sdw_upsampler_param_info(const sdw_upsampler* e, int index, const char** name, int64_t* numel);
+int sdw_upsampler_load_param(sdw_upsampler* e, const char* name, const void* src_f16, int64_t numel, void* stream);
+int sdw_upsampler_missing_params(const sdw_upsampler* e, const char** first_missing);
+/* in_u8 [frames][in_h][in_w][3] uint8 RGB -> out_u8 [frames][4 in_h][4 in_w][3] = round(clamp(y, 0, 1) * 255) with
+ * y = RRDBNet(fp16(u / 255)); out_preclamp_f32 (optional) fp32 [frames][4 in_h][4 in_w][3] = y.
+ * use_graph = 1 captures the GEMM sequence into a CUDA graph on first use (`stream` must be a real stream). */
+int sdw_upsampler_run(sdw_upsampler* e, const uint8_t* in_u8, uint8_t* out_u8, float* out_preclamp_f32, int use_graph,
+                      void* stream);
+/* tooling: CUDA-event time of every op of one run, written as TSV to `path` */
+int sdw_upsampler_debug_profile(sdw_upsampler* e, const char* path, void* stream);
+/* the upsampler's two edge convs (tests / tooling):
+ *   conv_first_u8 : y fp16 [B][H][W] at channel pitch ldy = 3x3 pad 1 conv of fp16(x / 255), x uint8 [B][H][W][3];
+ *                   w OIHW fp16 [N][3][3][3], bias fp32 [N] or null
+ *   conv_last_u8  : conv_out_small with nout = 3 and the post-process round(clamp(v, 0, 1) * 255) */
+int sdw_conv_first_u8(const uint8_t* x, int B, int H, int W, const void* w, const float* bias, int N, void* y, int64_t ldy,
+                      void* stream);
+int sdw_conv_last_u8(const void* x, int64_t ldx, int B, int H, int W, int C, const void* w, const float* bias,
+                     float* out_f32, uint8_t* out_u8, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Frame-sharded walk over the GPUs of one box (one process per GPU): the three exchanges of the path, as thin NCCL

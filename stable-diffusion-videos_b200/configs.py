@@ -202,3 +202,22 @@ def random_state_dict(shapes: Dict[str, tuple], seed: int, dtype=None, device="c
             t = (torch.rand(shp, generator=g) * 2 - 1) * bound
         sd[name] = t.to(dtype or torch.float16).to(device)
     return sd
+
+
+def esrgan_param_shapes(num_block=23, num_feat=64, num_grow_ch=32, num_in_ch=3, num_out_ch=3):
+    """basicsr RRDBNet (scale 4) state-dict keys and shapes, in registration order (16,697,987 parameters for the
+    23-block RealESRGAN_x4plus network)."""
+    shapes = {"conv_first.weight": (num_feat, num_in_ch, 3, 3), "conv_first.bias": (num_feat,)}
+    for i in range(num_block):
+        for r in range(1, 4):
+            for k in range(1, 6):
+                cin = num_feat + (k - 1) * num_grow_ch
+                cout = num_grow_ch if k < 5 else num_feat
+                shapes[f"body.{i}.rdb{r}.conv{k}.weight"] = (cout, cin, 3, 3)
+                shapes[f"body.{i}.rdb{r}.conv{k}.bias"] = (cout,)
+    for name in ("conv_body", "conv_up1", "conv_up2", "conv_hr"):
+        shapes[f"{name}.weight"] = (num_feat, num_feat, 3, 3)
+        shapes[f"{name}.bias"] = (num_feat,)
+    shapes["conv_last.weight"] = (num_out_ch, num_feat, 3, 3)
+    shapes["conv_last.bias"] = (num_out_ch,)
+    return shapes

@@ -52,8 +52,10 @@ struct EpiRow {
   const float* rowvec;
 };
 
-// fused epilogue of one accumulator (columns n_base .. n_base + BN) of this warpgroup's 64 rows
-template <int BN>
+// fused epilogue of one accumulator (columns n_base .. n_base + BN) of this warpgroup's 64 rows.  XE = 1 (the extended
+// epilogue of the Real-ESRGAN dense blocks): LeakyReLU(0.2), a scale on the residual and a second, unit-scale residual;
+// XE = 0 compiles the original epilogue unchanged.
+template <int BN, int XE>
 __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)[BN / 2], int n_base, const EpiRow (&R)[2],
                                               int lane, int wg, int lrow0, uint8_t* stage, uint64_t* res_full, int x0,
                                               int y0, int b0, uint32_t& chunk_count) {
@@ -85,7 +87,14 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)
     if (p.bias) o += __ldg(p.bias + n);
     if (p.rowvec) o += __ldg(R[h].rowvec + n);
     if (p.act == 1) o = silu_f(o);
+    if constexpr (XE != 0) {
+      if (p.act == 2) o = o > 0.f ? o : 0.2f * o;
+    }
     return o;
+  };
+  auto add_res = [&](float& o, float r) {
+    if constexpr (XE != 0) o = fmaf(p.res_scale, r, o);
+    else o += r;
   };
   // 2 x 2 values (rows h = 0 / 1, columns n, n + 1) of the plain path, residual added, stored or staged
   auto plain_pair = [&](int j, int n, uint8_t* staged, int scol) {
@@ -96,16 +105,25 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)
       if (staged && tma_res) {
         const float2 f =
             __half22float2(*reinterpret_cast<const __half2*>(staged + (lrow0 + 8 * h) * 64 + scol * 2));
-        o0 += f.x;
-        o1 += f.y;
+        add_res(o0, f.x);
+        add_res(o1, f.y);
       } else if (p.resid && R[h].ok) {
         if (vec2 && n + 1 < p.N) {
           const float2 f = __half22float2(*reinterpret_cast<const __half2*>(p.resid + R[h].res_off + n));
-          o0 += f.x;
-          o1 += f.y;
+          add_res(o0, f.x);
+          add_res(o1, f.y);
+          if (XE != 0 && p.resid2) {
+            const float2 g = __half22float2(*reinterpret_cast<const __half2*>(p.resid2 + R[h].res_off + n));
+            o0 += g.x;
+            o1 += g.y;
+          }
         } else {
-          if (n < p.N) o0 += __half2float(p.resid[R[h].res_off + n]);
-          if (n + 1 < p.N) o1 += __half2float(p.resid[R[h].res_off + n + 1]);
+          if (n < p.N) add_res(o0, __half2float(p.resid[R[h].res_off + n]));
+          if (n + 1 < p.N) add_res(o1, __half2float(p.resid[R[h].res_off + n + 1]));
+          if (XE != 0 && p.resid2) {
+            if (n < p.N) o0 += __half2float(p.resid2[R[h].res_off + n]);
+            if (n + 1 < p.N) o1 += __half2float(p.resid2[R[h].res_off + n + 1]);
+          }
         }
       }
       if (staged) {
@@ -225,7 +243,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)
   }
 }
 
-template <int BN, int NSUB, int TR, int CL>
+template <int BN, int NSUB, int TR, int CL, int XE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_constant__ GemmKParams p) {
   using Cfg = GemmCfg<BN, NSUB, TR>;
   constexpr int A_BYTES = Cfg::A_BYTES;
@@ -404,7 +422,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
       }
 #pragma unroll
       for (int sub = 0; sub < NSUB; ++sub)
-        gemm_epilogue<BN>(p, acc[sub], n0 + sub * BN, R, lane, wg, lrow0, stage_buf, res_full + 2 * wg, x0, y0, b0,
+        gemm_epilogue<BN, XE>(p, acc[sub], n0 + sub * BN, R, lane, wg, lrow0, stage_buf, res_full + 2 * wg, x0, y0, b0,
                           chunk_count);
     }
     if (p.epi_tma && (threadIdx.x & 127) == 0) bulk_wait_group<0>();  // every output chunk has reached global memory
@@ -581,7 +599,16 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
   // kernel version: CTA pairs (weight tile multicast to two M tiles) need >= 2 M tiles and a wide-enough N; batched
   // matmuls must pair within one (h, b)
   const int m_tiles = p.tiles_w * p.tiles_h * tiles_b;
+  SDW_REQUIRE(d.act >= 0 && d.act <= 2, "activation: 0 none, 1 SiLU, 2 LeakyReLU(0.2)");
+  SDW_REQUIRE(!d.resid2 || (d.resid && d.mode == GEMM_PLAIN), "a second residual needs the first one and the plain mode");
+  // the extended epilogue (LeakyReLU, residual scale, second residual) and BLOCK_N 32 exist as single-CTA kernels with
+  // BLOCK_N 32 / 64 only; every other descriptor plans exactly as before
+  const bool xe = d.act == 2 || d.res_scale != 1.f || d.resid2 != nullptr || d.bn == 32;
+  L->xe = xe ? 1 : 0;
+  if (xe) SDW_REQUIRE(d.ver != 2 && (d.bn == 0 || d.bn == 32 || d.bn == 64) && d.mode == GEMM_PLAIN && d.tr != 2 && d.nsub < 2,
+                      "BLOCK_N 32, LeakyReLU and the residual scales need single CTAs with BLOCK_N 32 or 64 (plain mode)");
   int ver = d.ver;
+  if (ver == 0 && xe) ver = 1;
   if (ver == 0) ver = (m_tiles >= 2 && d.N >= 128 && (!d.b_batched || p.tiles_w % 2 == 0)) ? 2 : 1;
   SDW_REQUIRE(ver == 1 || ver == 2, "unknown kernel version");
   if (ver == 2) SDW_REQUIRE(!d.b_batched || p.tiles_w % 2 == 0, "CTA-pair batched matmul needs an even tile count per row");
@@ -620,7 +647,7 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
     res_sW = rs ? d.r_sW : ldr;
     res_sH = rs ? d.r_sH : OW * ldr;
     res_sB = rs ? d.r_sB : OH * OW * ldr;
-    const bool res_ok = !d.resid || (d.mode == GEMM_PLAIN && ok16(d.resid) && ok_strides(res_sW, res_sH, res_sB));
+    const bool res_ok = !d.resid || (d.mode == GEMM_PLAIN && !d.resid2 && ok16(d.resid) && ok_strides(res_sW, res_sH, res_sB));
     can_tma = !d.b_batched && vt_ok && res_ok && (!d.rowvec || d.rowvec_ld == 0) && d.N % 8 == 0 && ncols > 0 &&
               ok16(d.out) && ok_strides(osW, osH, osB) && (!d.bias || ok16(d.bias));
     if (d.et == 2) SDW_REQUIRE(can_tma, "the TMA epilogue needs no per-sample row vector and 16-byte aligned views");
@@ -648,6 +675,7 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
     L->tr = 0;
   }
   const int m_tiles_f = p.tiles_w * p.tiles_h * ((d.B + bb - 1) / bb);
+  if (bn == 0 && xe) bn = 64;
   if (bn == 0) {
     static const int cand1[4] = {256, 160, 128, 64};
     static const int cand2[4] = {256, 192, 160, 128};
@@ -668,8 +696,8 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
       }
     }
   }
-  SDW_REQUIRE(bn == 64 || bn == 128 || bn == 160 || bn == 256 || (bn == 192 && ver == 2), "unsupported BLOCK_N");
-  if (ver == 2) SDW_REQUIRE(bn != 64, "the CTA-pair kernel needs BLOCK_N >= 128");
+  SDW_REQUIRE(bn == 32 || bn == 64 || bn == 128 || bn == 160 || bn == 256 || (bn == 192 && ver == 2), "unsupported BLOCK_N");
+  if (ver == 2) SDW_REQUIRE(bn != 32 && bn != 64, "the CTA-pair kernel needs BLOCK_N >= 128");
   if (d.ew == 4) SDW_REQUIRE(false, "one epilogue form on this GPU: epilogue width 4 is not available");
   SDW_REQUIRE(d.ew == 0 || d.ew == 2, "epilogue width must be 0 (auto) or 2");
   L->ew = 2;
@@ -748,6 +776,8 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
   p.rowvec = d.rowvec;
   p.rowvec_ld = d.rowvec_ld;
   p.resid = d.resid;
+  p.res_scale = d.res_scale;
+  p.resid2 = d.resid2;
   p.out = d.out;
   p.o_sW = osW;
   p.o_sH = osH;
@@ -757,7 +787,8 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
   p.r_sB = res_sB;
   // two-column (4-byte) output / residual accesses: every row offset and the column pair start even
   p.vec2 = ((p.o_sW | p.o_sH | p.o_sB) & 1) == 0 && (reinterpret_cast<uintptr_t>(d.out) & 3) == 0 &&
-           (!d.resid || (((p.r_sW | p.r_sH | p.r_sB) & 1) == 0 && (reinterpret_cast<uintptr_t>(d.resid) & 3) == 0));
+           (!d.resid || (((p.r_sW | p.r_sH | p.r_sB) & 1) == 0 && (reinterpret_cast<uintptr_t>(d.resid) & 3) == 0)) &&
+           (!d.resid2 || (reinterpret_cast<uintptr_t>(d.resid2) & 3) == 0);
   p.mode = d.mode;
   p.act = d.act;
   p.alpha = d.alpha;
@@ -770,11 +801,11 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
   return 0;
 }
 
-template <int BN, int NSUB, int TR, int CL>
+template <int BN, int NSUB, int TR, int CL, int XE = 0>
 static int launch_one(const GemmLaunch& l, cudaStream_t stream) {
   static int max_ctas = 0;  // CTAs of this kernel that can be resident at once (whole clusters)
   if (!max_ctas) {
-    SDW_CUDA_OK(cudaFuncSetAttribute(gemm_kernel<BN, NSUB, TR, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    SDW_CUDA_OK(cudaFuncSetAttribute(gemm_kernel<BN, NSUB, TR, CL, XE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      GEMM_SMEM_DYN));
     max_ctas = sm_count();
     if (CL > 1) {
@@ -792,21 +823,23 @@ static int launch_one(const GemmLaunch& l, cudaStream_t stream) {
       cfg.attrs = attr;
       cfg.numAttrs = 1;
       int nclusters = 0;
-      SDW_CUDA_OK(cudaOccupancyMaxActiveClusters(&nclusters, gemm_kernel<BN, NSUB, TR, CL>, &cfg));
+      SDW_CUDA_OK(cudaOccupancyMaxActiveClusters(&nclusters, gemm_kernel<BN, NSUB, TR, CL, XE>, &cfg));
       if (nclusters > 0) max_ctas = std::min(max_ctas, CL * nclusters);
     }
   }
   const dim3 grid(std::min<unsigned>(l.grid.x, static_cast<unsigned>(max_ctas)), 1, 1);
-  SDW_CUDA_OK(launch_cluster(gemm_kernel<BN, NSUB, TR, CL>, grid, dim3(GEMM_THREADS), GEMM_SMEM_DYN, stream, CL, l.p));
+  SDW_CUDA_OK(launch_cluster(gemm_kernel<BN, NSUB, TR, CL, XE>, grid, dim3(GEMM_THREADS), GEMM_SMEM_DYN, stream, CL, l.p));
   SDW_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
-// instantiations: single CTAs with BLOCK_N 64 / 128 / 160 / 256; CTA pairs with BLOCK_N 128 / 160 / 192 / 256 x
+// instantiations: single CTAs with BLOCK_N 64 / 128 / 160 / 256, and BLOCK_N 32 / 64 with the extended epilogue; CTA pairs with BLOCK_N 128 / 160 / 192 / 256 x
 // {per-tap, tap reuse} and one accumulator, 160 x 2 accumulators
 int launch_gemm(const GemmLaunch& l, cudaStream_t stream) {
-  const int key = l.ver * 100000 + l.bn * 100 + l.nsub * 10 + (l.tr ? 1 : 0);
+  const int key = l.xe * 1000000 + l.ver * 100000 + l.bn * 100 + l.nsub * 10 + (l.tr ? 1 : 0);
   switch (key) {
+    case 1103210: return launch_one<32, 1, 0, 1, 1>(l, stream);
+    case 1106410: return launch_one<64, 1, 0, 1, 1>(l, stream);
     case 106410: return launch_one<64, 1, 0, 1>(l, stream);
     case 112810: return launch_one<128, 1, 0, 1>(l, stream);
     case 116010: return launch_one<160, 1, 0, 1>(l, stream);

@@ -116,11 +116,13 @@ struct alignas(64) GemmKParams {
   int rowvec_ld;
   const __half* resid;      // residual or null; element offset = b*r_sB + oy'*r_sH + ox'*r_sW + n
   int64_t r_sW, r_sH, r_sB;
+  float res_scale;          // scale on the residual (1: plain add)
+  const __half* resid2;     // second, unit-scale residual with resid's strides, or null (direct-store epilogue only)
   __half* out;              // element offset = b*o_sB + (y*os+oy)*o_sH + (x*os+ox)*o_sW + n
   int64_t o_sW, o_sH, o_sB;
   int os, ox, oy;
   int mode;
-  int act;                  // 0 none, 1 SiLU
+  int act;                  // 0 none, 1 SiLU, 2 LeakyReLU(0.2)
   float alpha;              // scale on the accumulator (before bias)
   // GEMM_QKV_VT
   int vt_col0, vt_d, vt_heads, vt_ntok;
@@ -136,6 +138,7 @@ struct GemmLaunch {
   int nsub = 1;  // accumulators per activation tile (2 -> 128 x 2*BN tiles)
   int ew = 2;    // epilogue warps per 32 accumulator rows (always 2: each consumer warpgroup stores its own rows)
   int tr = 0;    // 1 -> tap-reuse mainloop (3x3 stride-1 convs)
+  int xe = 0;    // 1 -> extended epilogue (LeakyReLU, residual scale, second residual): single CTAs, BLOCK_N 32 / 64
 };
 
 // Describes one implicit GEMM in host terms; plan_gemm() turns it into a launch.
@@ -158,6 +161,8 @@ struct GemmDesc {
   const __half* resid = nullptr;
   int64_t ldr = 0;                 // residual pixel pitch (0 -> ldc); or explicit strides below
   int64_t r_sW = 0, r_sH = 0, r_sB = 0;
+  float res_scale = 1.f;           // out = act(alpha*acc + bias) + res_scale*resid + resid2
+  const __half* resid2 = nullptr;  // internal only (RRDB tail): same view as resid, needs resid, direct-store epilogue
   __half* out = nullptr;
   int64_t ldc = 0;                 // output pixel pitch; NHWC-contiguous output unless o_s* are given
   int64_t o_sW = 0, o_sH = 0, o_sB = 0;
@@ -167,7 +172,7 @@ struct GemmDesc {
   int vt_col0 = 0, vt_d = 0, vt_heads = 0, vt_ntok = 0;
   __half* vt = nullptr;
   int64_t vt_ld = 0;
-  int bn = 0;   // 0 = auto
+  int bn = 0;   // 0 = auto; 32 only when asked for, on single CTAs
   int ver = 0;  // 0 = auto, 1 / 2 force a kernel version
   int nsub = 0; // 0 = auto, 1 / 2: accumulators per activation tile (2: CTA-pair kernel, BLOCK_N 160)
   int ew = 0;   // 0 = auto or 2 (the only epilogue width of this kernel)
@@ -241,8 +246,12 @@ int layernorm(const __half* x, int64_t ldx, int64_t rows, int C, const float* ga
 int softmax_rows(__half* s, int64_t ld, int64_t rows, int n, cudaStream_t stream);
 int conv_in_small(const __half* x, int64_t ldx, int B, int H, int W, int Cin, const __half* w, const float* bias,
                   int N, __half* y, int64_t ldy, cudaStream_t stream);
+// post = 0: the VAE's uint8 post-process round(clamp(v/2 + 0.5, 0, 1) * 255); post = 1: round(clamp(v, 0, 1) * 255)
 int conv_out_small(const __half* x, int64_t ldx, int B, int H, int W, int C, const __half* w, const float* bias,
-                   int nout, float* out_f32, uint8_t* out_u8, cudaStream_t stream);
+                   int nout, float* out_f32, uint8_t* out_u8, cudaStream_t stream, int post = 0);
+// Real-ESRGAN conv_first: uint8 RGB [B][H][W][3] read as fp16(u / 255) -> 3x3 pad 1 -> N fp16 channels at pitch ldy
+int conv_first_u8(const uint8_t* x, int B, int H, int W, const __half* w, const float* bias, int N, __half* y,
+                  int64_t ldy, cudaStream_t stream);
 int vae_in(const float* x, float inv_scale, const __half* w, const float* bias, int F, int C, int H, int W, __half* z,
            cudaStream_t stream);
 int linear_f32(const float* in, int64_t ldi, const __half* w, const float* bias, int M, int N, int K, int silu_in,

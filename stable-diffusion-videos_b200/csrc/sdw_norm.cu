@@ -550,18 +550,25 @@ int softmax_rows(__half* s, int64_t ld, int64_t rows, int n, cudaStream_t stream
 }
 
 // =============================================================================================
-// conv_in: 3x3 pad 1, tiny Cin (4) -> N channels.  Block = N threads (one output channel each, weights in
-// registers), loops over a tile of pixels whose 3x3xCin patches sit in shared memory.
+// conv_in: 3x3 pad 1, tiny Cin (4: latents, 3: RGB) -> N channels.  Block = N threads (one output channel each, weights
+// in registers), loops over a tile of pixels whose 3x3xCin patches sit in shared memory.
 // w layout: [N][Cin][3][3] fp16 (the checkpoint's OIHW), bias fp32.
+// Input: fp16 activations, or uint8 RGB read as fp16(u / 255) (Real-ESRGAN's conv_first on an 8-bit frame).
 // =============================================================================================
-template <int CIN>
-__global__ void __launch_bounds__(512) conv_in_kernel(const __half* __restrict__ x, int64_t ldx, int B, int H, int W,
+__device__ __forceinline__ float conv_in_load(const __half* x, int64_t i) { return __half2float(x[i]); }
+__device__ __forceinline__ float conv_in_load(const uint8_t* x, int64_t i) {
+  return __half2float(__float2half_rn(static_cast<float>(x[i]) / 255.f));
+}
+
+template <int CIN, typename TIn>
+__global__ void __launch_bounds__(512) conv_in_kernel(const TIn* __restrict__ x, int64_t ldx, int B, int H, int W,
                                                        const __half* __restrict__ w, const float* __restrict__ bias,
                                                        int N, __half* __restrict__ y, int64_t ldy,
                                                        int pix_per_block) {
   // patch[pair][k] = (x of pixel 2*pair, x of pixel 2*pair + 1) for the 9*CIN taps: one 16-byte broadcast read feeds two
-  // FMAs on fp32 pairs (two taps x two pixels); thread = output channel, its 9*CIN weights live in registers
-  constexpr int K = 9 * CIN;
+  // FMAs on fp32 pairs (two taps x two pixels); thread = output channel, its 9*CIN weights live in registers.  An odd
+  // tap count is padded by one zero tap (zero input, zero weight) so the pairs stay 16-byte aligned.
+  constexpr int K = (9 * CIN + 1) & ~1;
   extern __shared__ float2 patch2[];  // [pix_per_block / 2][K]
   const int64_t P = static_cast<int64_t>(B) * H * W;
   const int64_t p0 = static_cast<int64_t>(blockIdx.x) * pix_per_block;
@@ -569,18 +576,19 @@ __global__ void __launch_bounds__(512) conv_in_kernel(const __half* __restrict__
   pdl_wait();
   pdl_launch_dependents();
   for (int i = threadIdx.x; i < pix_per_block * K; i += blockDim.x) {
-    const int c = i % CIN;
-    const int tap = (i / CIN) % 9;
+    const int k = i % K;
+    const int c = k % CIN;
+    const int tap = k / CIN;
     const int lp = i / K;
     const int64_t p = p0 + lp;
     float v = 0.f;
-    if (lp < np) {
+    if (lp < np && tap < 9) {
       const int xw = static_cast<int>(p % W), yh = static_cast<int>((p / W) % H);
       const int64_t b = p / (static_cast<int64_t>(W) * H);
       const int yy = yh + tap / 3 - 1, xx = xw + tap % 3 - 1;
-      if (yy >= 0 && yy < H && xx >= 0 && xx < W) v = __half2float(x[((b * H + yy) * W + xx) * ldx + c]);
+      if (yy >= 0 && yy < H && xx >= 0 && xx < W) v = conv_in_load(x, ((b * H + yy) * W + xx) * ldx + c);
     }
-    reinterpret_cast<float*>(patch2)[((lp >> 1) * K + tap * CIN + c) * 2 + (lp & 1)] = v;
+    reinterpret_cast<float*>(patch2)[((lp >> 1) * K + k) * 2 + (lp & 1)] = v;
   }
   __syncthreads();
   const int n = threadIdx.x;
@@ -593,6 +601,8 @@ __global__ void __launch_bounds__(512) conv_in_kernel(const __half* __restrict__
       const float wv = __half2float(w[(static_cast<int64_t>(n) * CIN + c) * 9 + tap]);
       wr[tap * CIN + c] = pk2(wv, wv);
     }
+#pragma unroll
+  for (int k = 9 * CIN; k < K; ++k) wr[k] = pk2(0.f, 0.f);
   const float bn = bias ? bias[n] : 0.f;
   for (int pr = 0; pr * 2 < np; ++pr) {
     uint64_t acc = pk2(bn, bn);
@@ -617,8 +627,21 @@ int conv_in_small(const __half* x, int64_t ldx, int B, int H, int W, int Cin, co
   const int ppb = 64;
   const int64_t P = static_cast<int64_t>(B) * H * W;
   const int threads = (N + 31) / 32 * 32;
-  conv_in_kernel<4><<<static_cast<unsigned>((P + ppb - 1) / ppb), threads, ppb * 36 * sizeof(float), stream>>>(
+  conv_in_kernel<4, __half><<<static_cast<unsigned>((P + ppb - 1) / ppb), threads, ppb * 36 * sizeof(float), stream>>>(
       x, ldx, B, H, W, w, bias, N, y, ldy, ppb);
+  SDW_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int conv_first_u8(const uint8_t* x, int B, int H, int W, const __half* w, const float* bias, int N, __half* y,
+                  int64_t ldy, cudaStream_t stream) {
+  SDW_REQUIRE(x && w && y && B > 0 && H > 0 && W > 0, "conv_first: null / empty");
+  SDW_REQUIRE(N >= 1 && N <= 512, "conv_first: 1 <= N <= 512");
+  const int ppb = 64;
+  const int64_t P = static_cast<int64_t>(B) * H * W;
+  const int threads = (N + 31) / 32 * 32;
+  conv_in_kernel<3, uint8_t><<<static_cast<unsigned>((P + ppb - 1) / ppb), threads, ppb * 28 * sizeof(float), stream>>>(
+      x, 3, B, H, W, w, bias, N, y, ldy, ppb);
   SDW_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -628,6 +651,7 @@ int conv_in_small(const __half* x, int64_t ldx, int B, int H, int W, int Cin, co
 // Input is the already normalised + SiLU'd fp16 NHWC tensor.  w layout: OIHW fp16 [NOUT][C][3][3].
 //   out_f32  : fp32 NHWC [P][NOUT] (UNet eps)          — optional
 //   out_u8   : uint8 NHWC [P][NOUT] = round(clamp(v/2+0.5,0,1)*255) (VAE frame; P:435-438 + numpy_to_pil) — optional
+//              with post = 1: round(clamp(v,0,1)*255) (Real-ESRGAN's conv_last, whose output is already in [0, 1])
 // =============================================================================================
 // A block owns a TS x TS pixel tile: its (TS+2)^2 halo is staged once in shared memory (the row-per-warp version
 // re-read every input pixel nine times from L2), the
@@ -636,7 +660,7 @@ template <int NOUT, int TS>
 __global__ void __launch_bounds__(256) conv_out_kernel(const __half* __restrict__ x, int64_t ldx, int B, int H, int W,
                                                        int C, const __half* __restrict__ w,
                                                        const float* __restrict__ bias, float* __restrict__ out_f32,
-                                                       uint8_t* __restrict__ out_u8) {
+                                                       uint8_t* __restrict__ out_u8, int post) {
   constexpr int HT = TS + 2;
   extern __shared__ __align__(16) uint8_t co_smem[];
   __half* halo = reinterpret_cast<__half*>(co_smem);  // [HT*HT][C]
@@ -746,7 +770,7 @@ __global__ void __launch_bounds__(256) conv_out_kernel(const __half* __restrict_
             const float v = acc[j][n] + (bias ? bias[n] : 0.f);
             if (out_f32) out_f32[p * NOUT + n] = v;
             if (out_u8) {
-              const float q = fminf(fmaxf(v * 0.5f + 0.5f, 0.f), 1.f);
+              const float q = fminf(fmaxf(post ? v : v * 0.5f + 0.5f, 0.f), 1.f);
               out_u8[p * NOUT + n] = static_cast<uint8_t>(rintf(q * 255.f));
             }
           }
@@ -759,7 +783,7 @@ __global__ void __launch_bounds__(256) conv_out_kernel(const __half* __restrict_
 
 template <int NOUT, int TS>
 static int launch_conv_out(const __half* x, int64_t ldx, int B, int H, int W, int C, const __half* w, const float* bias,
-                           float* out_f32, uint8_t* out_u8, cudaStream_t stream) {
+                           float* out_f32, uint8_t* out_u8, int post, cudaStream_t stream) {
   const size_t smem = (static_cast<size_t>((TS + 2) * (TS + 2)) + NOUT * 9) * C * sizeof(__half);
   SDW_REQUIRE(smem <= 227 * 1024, "conv_out: channel count too large for the halo tile");
   static bool attr_done = false;
@@ -769,22 +793,24 @@ static int launch_conv_out(const __half* x, int64_t ldx, int B, int H, int W, in
   }
   const int64_t tiles = static_cast<int64_t>(B) * ((H + TS - 1) / TS) * ((W + TS - 1) / TS);
   const int64_t blocks = std::min<int64_t>(tiles, static_cast<int64_t>(sm_count()) * 2);  // persistent: the weights are staged once per block
-  conv_out_kernel<NOUT, TS><<<static_cast<unsigned>(blocks), 256, smem, stream>>>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8);
+  conv_out_kernel<NOUT, TS><<<static_cast<unsigned>(blocks), 256, smem, stream>>>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8,
+                                                                                  post);
   SDW_CUDA_OK(cudaGetLastError());
   return 0;
 }
 
 int conv_out_small(const __half* x, int64_t ldx, int B, int H, int W, int C, const __half* w, const float* bias,
-                   int nout, float* out_f32, uint8_t* out_u8, cudaStream_t stream) {
+                   int nout, float* out_f32, uint8_t* out_u8, cudaStream_t stream, int post) {
   SDW_REQUIRE(nout == 3 || nout == 4, "conv_out: 3 or 4 output channels");
+  SDW_REQUIRE(post == 0 || post == 1, "conv_out: post-process 0 (v/2 + 0.5) or 1 (v)");
   SDW_REQUIRE(C % 8 == 0 && ldx % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0, "conv_out: 16-byte aligned channel rows");
   // 16 x 16 tiles when their halo fits comfortably (C <= 128), 8 x 8 otherwise
   const bool big = C <= 128 && H >= 16 && W >= 16;
   if (nout == 4)
-    return big ? launch_conv_out<4, 16>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8, stream)
-               : launch_conv_out<4, 8>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8, stream);
-  return big ? launch_conv_out<3, 16>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8, stream)
-             : launch_conv_out<3, 8>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8, stream);
+    return big ? launch_conv_out<4, 16>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8, post, stream)
+               : launch_conv_out<4, 8>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8, post, stream);
+  return big ? launch_conv_out<3, 16>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8, post, stream)
+             : launch_conv_out<3, 8>(x, ldx, B, H, W, C, w, bias, out_f32, out_u8, post, stream);
 }
 
 // =============================================================================================
