@@ -212,7 +212,7 @@ int sdw_attention(const void* q, int64_t q_ld, const void* k, int64_t k_ld, cons
 
 /* normalisation layers (tests / tooling).  x, y: fp16 [B][P][ld] NHWC views (ld = channel pitch, multiple of 8);
  * GroupNorm over (P pixels x C/G channels) per sample with optional SiLU; LayerNorm over the C channels of each row.
- * gamma / beta fp32 [C]. */
+ * gamma / beta fp32 [C].  LayerNorm also needs x, y, gamma and beta 16-byte aligned (it returns 1 otherwise). */
 int sdw_groupnorm(const void* x, int64_t ldx, int B, int64_t P, int C, int G, const float* gamma, const float* beta,
                   float eps, int silu, void* y, int64_t ldy, void* stream);
 int sdw_layernorm(const void* x, int64_t ldx, int64_t rows, int C, const float* gamma, const float* beta, float eps,
@@ -278,6 +278,16 @@ int sdw_clip_missing_params(const sdw_clip* e, const char** first_missing);
 /* ids: device int32 [B][max_positions] (token ids, already padded / truncated by the tokenizer);
  * out: device fp16 [B][max_positions][hidden] = last_hidden_state after the final LayerNorm */
 int sdw_clip_forward(sdw_clip* e, const int32_t* ids, int B, void* out_f16, void* stream);
+/* the tower's own kernels, one entry point each (tests / tooling); all tensors fp16 unless stated:
+ *   clip_embed     : x [rows][H] = fp16(fp32(tok[clamp(ids[r], 0, vocab-1)]) + fp32(pos[r % P])), ids device int32
+ *                    [rows], tok [vocab][H], pos [P][H]; H % 8 == 0.  Out-of-range ids are clamped, not rejected.
+ *   clip_attention : causal softmax(q k^T / 8) v per (sample, head); qkv [B][P][3H] (q | k | v column blocks, head h at
+ *                    columns h*64), out [B][P][H], H = 64 heads, 1 <= P <= 96
+ *   clip_act       : in place over n values: gelu_erf = 0 quick-GELU x sigmoid(1.702 x), 1 erf GELU */
+int sdw_clip_embed(const int32_t* ids, const void* tok, const void* pos, int rows, int P, int H, int vocab, void* x,
+                   void* stream);
+int sdw_clip_attention(const void* qkv, int B, int P, int heads, void* out, void* stream);
+int sdw_clip_act(void* x, int64_t n, int gelu_erf, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Real-ESRGAN x4 upsampler: replaces `self.upsampler(image)` of make_clip_frames(upsample=True)

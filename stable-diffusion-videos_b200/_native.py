@@ -132,3 +132,23 @@ def layernorm(x, rows, Cc, gamma, beta, eps, y):
 
 def gemm(desc):
     check(lib().sdw_gemm(C.byref(desc), stream_ptr()))
+
+
+def clip_embed(ids, tok, pos, rows, P, x):
+    """x fp16 [rows][H] = tok[clamp(ids[r], 0, vocab - 1)] + pos[r % P]; ids int32 [rows], tok [vocab][H], pos [P][H]."""
+    require_cuda(ids, tok, pos, x)
+    vocab, H = tok.shape
+    check(lib().sdw_clip_embed(ptr(ids), ptr(tok), ptr(pos), C.c_int(rows), C.c_int(P), C.c_int(H), C.c_int(vocab),
+                               ptr(x), stream_ptr()))
+
+
+def clip_attention(qkv, B, P, heads, out):
+    """causal attention of the CLIP tower: qkv fp16 [B][P][3 * 64 heads] -> out fp16 [B][P][64 heads]."""
+    require_cuda(qkv, out)
+    check(lib().sdw_clip_attention(ptr(qkv), C.c_int(B), C.c_int(P), C.c_int(heads), ptr(out), stream_ptr()))
+
+
+def clip_act(x, n, gelu_erf):
+    """in place over the first n fp16 values of x: quick-GELU (gelu_erf = 0) or erf GELU (1)."""
+    require_cuda(x)
+    check(lib().sdw_clip_act(ptr(x), C.c_int64(n), C.c_int(int(gelu_erf)), stream_ptr()))

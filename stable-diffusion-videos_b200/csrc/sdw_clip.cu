@@ -100,7 +100,8 @@ __global__ void clip_act_kernel(__half* __restrict__ x, int64_t n, int gelu_erf)
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float v = __half2float(x[i]);
-  const float y = gelu_erf ? 0.5f * v * (1.f + erff(v * 0.70710678118654752f)) : v / (1.f + __expf(-1.702f * v));
+  // erf GELU as 0.5 v erfc(-v / sqrt 2): 1 + erf(x) cancels for x < -2 and loses up to 2 fp16 ulps of the result
+  const float y = gelu_erf ? 0.5f * v * erfcf(v * -0.70710678118654752f) : v / (1.f + __expf(-1.702f * v));
   x[i] = __float2half_rn(y);
 }
 
@@ -313,6 +314,39 @@ int sdw_clip_forward(sdw_clip* e, const int32_t* ids, int B, void* out_f16, void
     std::swap(x, y);
   }
   return layernorm(x, H, T, H, E->lnf_g, E->lnf_b, c.eps, static_cast<__half*>(out_f16), H, st);
+}
+
+// the tower's three kernels on their own (tests / tooling)
+int sdw_clip_embed(const int32_t* ids, const void* tok, const void* pos, int rows, int P, int H, int vocab, void* x,
+                   void* stream) {
+  SDW_REQUIRE(ids && tok && pos && x, "null");
+  SDW_REQUIRE(rows >= 1 && P >= 1 && vocab >= 1 && H >= 8 && H % 8 == 0, "CLIP embedding: rows, P, vocab >= 1, H % 8 == 0");
+  SDW_REQUIRE(((reinterpret_cast<uintptr_t>(tok) | reinterpret_cast<uintptr_t>(pos) | reinterpret_cast<uintptr_t>(x)) & 3) == 0,
+              "CLIP embedding: tok, pos and x must be 4-byte aligned");
+  clip_embed_kernel<<<static_cast<unsigned>(rows), 128, 0, static_cast<cudaStream_t>(stream)>>>(
+      ids, static_cast<const __half*>(tok), static_cast<const __half*>(pos), P, H, vocab, static_cast<__half*>(x));
+  SDW_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int sdw_clip_attention(const void* qkv, int B, int P, int heads, void* out, void* stream) {
+  SDW_REQUIRE(qkv && out, "null");
+  SDW_REQUIRE(P >= 1 && P <= 96, "CLIP attention: 1 <= P <= 96 (the kernel stages K and V of 96 positions)");
+  SDW_REQUIRE(B >= 1 && B <= 65535 && heads >= 1 && heads <= 65535, "CLIP attention: bad B / heads");
+  clip_attn_kernel<96><<<dim3(heads, B), 128, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const __half*>(qkv), P, heads * 64, static_cast<__half*>(out));
+  SDW_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+int sdw_clip_act(void* x, int64_t n, int gelu_erf, void* stream) {
+  SDW_REQUIRE(x && n >= 0 && (gelu_erf == 0 || gelu_erf == 1), "CLIP activation: null x, n < 0 or bad activation");
+  SDW_REQUIRE(n <= int64_t(1) << 38, "CLIP activation: n too large for one launch");
+  if (n == 0) return 0;
+  clip_act_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<__half*>(x), n, gelu_erf);
+  SDW_CUDA_OK(cudaGetLastError());
+  return 0;
 }
 
 }  // extern "C"

@@ -457,13 +457,17 @@ static int launch_ln_c40(const __half* x, int64_t ldx, int64_t rows, const float
 int layernorm(const __half* x, int64_t ldx, int64_t rows, int C, const float* gamma, const float* beta, float eps,
               __half* y, int64_t ldy, cudaStream_t stream) {
   SDW_REQUIRE(C % 8 == 0 && C <= 8 * 32 * 8, "LayerNorm: C % 8 == 0 and C <= 2048");
+  // both kernels move x / y in 16-byte vectors and gamma / beta in float4s
+  SDW_REQUIRE(ldx % 8 == 0 && ldy % 8 == 0, "LayerNorm: row pitch must be a multiple of 8");
+  SDW_REQUIRE(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0,
+              "LayerNorm: x and y must be 16-byte aligned");
+  SDW_REQUIRE(((reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15) == 0,
+              "LayerNorm: gamma and beta must be 16-byte aligned");
   const int vecs = C / 8;
   const int rev = norm_reverse();
   // the UNet widths take the lane-group kernel; SDW_LN_C40=0 keeps the generic one (A/B)
   static const int c40_env = [] { const char* e = std::getenv("SDW_LN_C40"); return e ? std::atoi(e) : 1; }();
-  const bool vec_ok = (ldx % 8 == 0) && (ldy % 8 == 0) && ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0 &&
-                      ((reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta)) & 15) == 0;
-  if (c40_env && vec_ok) {
+  if (c40_env) {
     if (C == 320) return launch_ln_c40<8>(x, ldx, rows, gamma, beta, eps, y, ldy, rev, stream);
     if (C == 640) return launch_ln_c40<16>(x, ldx, rows, gamma, beta, eps, y, ldy, rev, stream);
     if (C == 1280) return launch_ln_c40<32>(x, ldx, rows, gamma, beta, eps, y, ldy, rev, stream);

@@ -21,6 +21,38 @@ def test_every_declared_symbol_is_exported():
     assert lib.sdw_abi_version() == 2
 
 
+def test_layernorm_rejects_pitches_and_pointers_its_kernels_cannot_load():
+    """both LayerNorm kernels load x in 16-byte vectors and gamma / beta as float4s: a pitch that is not a multiple of 8
+    or a misaligned pointer is an argument error, returned before anything is launched (the addresses are fake and
+    never dereferenced)."""
+    from stable_diffusion_videos_b200 import _native
+
+    lib = _native.lib()
+    x, y, g, b = (C.c_void_p(k << 30) for k in (1, 2, 3, 4))
+    I64, F = C.c_int64, C.c_float
+    assert lib.sdw_layernorm(x, I64(321), I64(77), 320, g, b, F(1e-5), y, I64(320), None) == 1
+    assert b"row pitch must be a multiple of 8" in lib.sdw_last_error()
+    assert lib.sdw_layernorm(x, I64(768), I64(77), 768, g, b, F(1e-5), y, I64(770), None) == 1
+    assert b"row pitch must be a multiple of 8" in lib.sdw_last_error()
+    assert lib.sdw_layernorm(x, I64(768), I64(77), 768, C.c_void_p((3 << 30) + 4), b, F(1e-5), y, I64(768), None) == 1
+    assert b"gamma and beta must be 16-byte aligned" in lib.sdw_last_error()
+    assert lib.sdw_layernorm(C.c_void_p((1 << 30) + 8), I64(768), I64(77), 768, g, b, F(1e-5), y, I64(768), None) == 1
+    assert b"x and y must be 16-byte aligned" in lib.sdw_last_error()
+
+
+def test_clip_kernel_entry_points_reject_bad_arguments():
+    """the CLIP kernels' entry points validate before launching (fake addresses, never dereferenced)"""
+    from stable_diffusion_videos_b200 import _native
+
+    lib = _native.lib()
+    p = C.c_void_p(1 << 30)
+    assert lib.sdw_clip_attention(p, 1, 97, 12, p, None) == 1  # K / V of at most 96 positions fit the shared memory
+    assert b"P <= 96" in lib.sdw_last_error()
+    assert lib.sdw_clip_attention(p, 1, 0, 12, p, None) == 1
+    assert lib.sdw_clip_embed(p, p, p, 77, 77, 100, 1000, p, None) == 1  # H % 8
+    assert lib.sdw_clip_act(p, C.c_int64(10), 2, None) == 1
+
+
 def test_engine_dry_run_sizes_sd14_arena():
     from stable_diffusion_videos_b200 import _native
     from stable_diffusion_videos_b200.configs import UNetConfig, VAEConfig

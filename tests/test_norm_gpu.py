@@ -56,7 +56,9 @@ def test_groupnorm_strided_views_and_determinism():
     assert (outs[0].float() - ref).abs().max().item() <= 2 ** -9 * ref.abs().max().item() + 1e-3
 
 
-@pytest.mark.parametrize("rows,Cc", [(4096, 320), (1000, 640), (77, 1280), (5, 512), (4099, 320), (3, 320), (1, 640), (129, 768)])
+@pytest.mark.parametrize("rows,Cc", [(4096, 320), (1000, 640), (77, 1280), (5, 512), (4099, 320), (3, 320), (1, 640), (129, 768)] +
+                         # the CLIP widths: OpenCLIP-H (1024, five vectors per lane) and the 8-vector kernel (1288, 2048)
+                         [(r, c) for c in (1024, 1288, 2048) for r in (77, 154, 616)])
 def test_layernorm(rows, Cc):
     n = _native()
     x = _rand(rows, Cc, seed=5, scale=2.0, shift=-0.5)
@@ -65,8 +67,8 @@ def test_layernorm(rows, Cc):
     y = torch.full_like(x, float("nan"))
     n.layernorm(x, rows, Cc, gamma, beta, 1e-5, y)
     torch.cuda.synchronize()
-    ref = Fn.layer_norm(x.float(), (Cc,), gamma, beta, 1e-5)
-    assert (y.float() - ref).abs().max().item() <= 2 ** -9 * ref.abs().max().item() + 1e-3
+    ref = Fn.layer_norm(x.double(), (Cc,), gamma.double(), beta.double(), 1e-5)
+    assert (y.double() - ref).abs().max().item() <= 2 ** -9 * ref.abs().max().item() + 1e-3
 
 
 @pytest.mark.parametrize("Cc", [320, 640, 1280])
@@ -130,7 +132,7 @@ def test_groupnorm_group_counts_and_tiny_images(B, H, W, Cc, G, silu):
     assert (y.double() - ref).abs().max().item() <= 2 ** -9 * ref.abs().max().item() + 1e-3
 
 
-@pytest.mark.parametrize("Cc", [320, 768])
+@pytest.mark.parametrize("Cc", [320, 768, 1024, 1288, 2048])
 @pytest.mark.parametrize("offset", [0, 64, 256, 512])
 def test_layernorm_large_mean(offset, Cc):
     """the same offset sweep for LayerNorm (two-pass statistics)"""
