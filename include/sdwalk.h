@@ -120,6 +120,11 @@ int sdw_engine_create(const sdw_engine_config* cfg, sdw_engine** out);
 void sdw_engine_destroy(sdw_engine* e);
 int sdw_engine_arena_bytes(const sdw_engine* e, uint64_t* bytes);
 int sdw_engine_bind(sdw_engine* e, void* arena, uint64_t bytes);
+/* The parameter table, the same for all three engines (sampler, CLIP tower, upsampler): param_info enumerates index
+ * 0 .. num_params-1 in the engine's registration order (for this engine, not alphabetically: the key set is that of the
+ * checkpoint).  load_param returns 1 without launching anything when the engine is not bound, the name is unknown or
+ * numel differs, with a message naming the parameter.  missing_params counts the parameters not loaded yet and names
+ * the first in `first_missing`; it returns -1 for a null engine. */
 int sdw_engine_num_params(const sdw_engine* e);
 int sdw_engine_param_info(const sdw_engine* e, int index, const char** name, int64_t* numel);
 /* src: fp16 device tensor in the checkpoint's own layout (OIHW conv / [out,in] linear / vectors) */
@@ -271,6 +276,7 @@ int sdw_clip_create(const sdw_clip_config* cfg, sdw_clip** out);
 void sdw_clip_destroy(sdw_clip* e);
 int sdw_clip_arena_bytes(const sdw_clip* e, uint64_t* bytes);
 int sdw_clip_bind(sdw_clip* e, void* arena, uint64_t bytes);
+/* parameter table as the sampler engine's */
 int sdw_clip_num_params(const sdw_clip* e);
 int sdw_clip_param_info(const sdw_clip* e, int index, const char** name, int64_t* numel);
 int sdw_clip_load_param(sdw_clip* e, const char* name, const void* data_f16, int64_t numel, void* stream);
@@ -307,6 +313,7 @@ int sdw_upsampler_create(const sdw_upsampler_config* cfg, sdw_upsampler** out);
 void sdw_upsampler_destroy(sdw_upsampler* e);
 int sdw_upsampler_arena_bytes(const sdw_upsampler* e, uint64_t* bytes);
 int sdw_upsampler_bind(sdw_upsampler* e, void* arena, uint64_t bytes);
+/* parameter table as the sampler engine's */
 int sdw_upsampler_num_params(const sdw_upsampler* e);
 int sdw_upsampler_param_info(const sdw_upsampler* e, int index, const char** name, int64_t* numel);
 int sdw_upsampler_load_param(sdw_upsampler* e, const char* name, const void* src_f16, int64_t numel, void* stream);

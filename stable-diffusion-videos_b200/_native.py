@@ -75,6 +75,71 @@ def require_cuda(*tensors):
             raise SdwError("libsdwalk operates on CUDA tensors only (no CPU fallback)")
 
 
+class NativeModel:
+    """One native engine behind the `sdw_<prefix>_*` functions (engine, clip, upsampler): created from its config
+    struct, bound to a zero-filled arena on `device` aligned to `align` bytes, destroyed with this object.  `h` is the
+    handle the engine's own entry points take; `what` names the model in error messages."""
+
+    def __init__(self, prefix, cfg, align, device, what):
+        self.prefix, self.device, self.what = prefix, torch.device(device), what
+        self._fn("destroy").restype = None
+        self.h = C.c_void_p()
+        check(self._fn("create")(C.byref(cfg), C.byref(self.h)))
+        nbytes = C.c_uint64()
+        check(self._fn("arena_bytes")(self.h, C.byref(nbytes)))
+        self.arena_bytes = int(nbytes.value)
+        with torch.cuda.device(self.device):
+            self.arena = torch.zeros(self.arena_bytes + align, dtype=torch.uint8, device=self.device)
+            base = (self.arena.data_ptr() + align - 1) // align * align
+            check(self._fn("bind")(self.h, C.c_void_p(base), C.c_uint64(self.arena_bytes)))
+
+    def _fn(self, name):
+        return getattr(lib(), f"sdw_{self.prefix}_{name}")
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                self._fn("destroy")(self.h)
+                self.h = None
+        except Exception:
+            pass
+
+    def param_names(self):
+        """{name: numel} of every parameter, in the engine's registration order."""
+        name, numel, out = C.c_char_p(), C.c_int64(), {}
+        for i in range(self._fn("num_params")(self.h)):
+            check(self._fn("param_info")(self.h, i, C.byref(name), C.byref(numel)))
+            out[name.value.decode()] = int(numel.value)
+        return out
+
+    def load(self, items, strict=True):
+        """Load {name: tensor} (any device / dtype, handed over as contiguous fp16) and require that every parameter is
+        then loaded.  Unknown names raise when `strict` (else they are skipped) and element counts are checked, all
+        before anything is loaded."""
+        expected = self.param_names()
+        todo = []
+        for name, t in items.items():
+            if name not in expected:
+                if strict:
+                    raise SdwError(f"unexpected {self.what} parameter {name}")
+                continue
+            if t.numel() != expected[name]:
+                raise SdwError(f"shape mismatch for {name}: {tuple(t.shape)} has {t.numel()} elements, "
+                               f"expected {expected[name]}")
+            todo.append((name, t))
+        keep = []  # the fp16 copies stay alive until the loads on the stream have run
+        with torch.cuda.device(self.device):
+            for name, t in todo:
+                th = t.detach().to(device=self.device, dtype=torch.float16).contiguous()
+                keep.append(th)
+                check(self._fn("load_param")(self.h, name.encode(), ptr(th), C.c_int64(th.numel()), stream_ptr()))
+            torch.cuda.current_stream().synchronize()
+        first = C.c_char_p()
+        missing = self._fn("missing_params")(self.h, C.byref(first))
+        if missing:
+            raise SdwError(f"{missing} {self.what} parameters not loaded (first: {first.value.decode()})")
+
+
 # ----------------------------------------------------------------------------------------------
 def slerp_lerp_batch(lat_a, lat_b, emb_a, emb_b, t, dot_threshold=0.9995):
     """Batched generate_inputs math (stable_diffusion_pipeline.py:466-468): returns (latents[n], embeds[n])."""

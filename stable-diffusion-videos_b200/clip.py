@@ -31,24 +31,8 @@ class NativeCLIPTextEncoder:
         c = ClipConfig(vocab_size, max_position_embeddings, hidden_size, num_hidden_layers, num_attention_heads,
                        intermediate_size, int(hidden_act == "gelu"), layer_norm_eps, max_batch)
         self.cfg = c
-        lib = N.lib()
-        lib.sdw_clip_destroy.restype = None
-        self._h = C.c_void_p()
-        N.check(lib.sdw_clip_create(C.byref(c), C.byref(self._h)))
-        nbytes = C.c_uint64()
-        N.check(lib.sdw_clip_arena_bytes(self._h, C.byref(nbytes)))
-        with torch.cuda.device(self.device):
-            self.arena = torch.zeros(int(nbytes.value) + 256, dtype=torch.uint8, device=self.device)
-            base = (self.arena.data_ptr() + 255) // 256 * 256
-            N.check(lib.sdw_clip_bind(self._h, C.c_void_p(base), C.c_uint64(int(nbytes.value))))
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                N.lib().sdw_clip_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        self._model = N.NativeModel("clip", c, 256, self.device, "CLIP")
+        self._h = self._model.h
 
     # ------------------------------------------------------------------------------------------
     @classmethod
@@ -61,36 +45,11 @@ class NativeCLIPTextEncoder:
         return enc
 
     def param_names(self):
-        lib = N.lib()
-        name, numel, out = C.c_char_p(), C.c_int64(), {}
-        for i in range(lib.sdw_clip_num_params(self._h)):
-            N.check(lib.sdw_clip_param_info(self._h, i, C.byref(name), C.byref(numel)))
-            out[name.value.decode()] = int(numel.value)
-        return out
+        return self._model.param_names()
 
     def load_state_dict(self, sd, strict=True):
-        lib = N.lib()
-        expected = self.param_names()
-        keep = []
-        with torch.cuda.device(self.device):
-            for name, t in sd.items():
-                if name.endswith("position_ids"):
-                    continue  # a buffer, not a parameter
-                if name not in expected:
-                    if strict:
-                        raise N.SdwError(f"unexpected CLIP parameter {name}")
-                    continue
-                if t.numel() != expected[name]:
-                    raise N.SdwError(f"shape mismatch for {name}: {tuple(t.shape)} has {t.numel()} elements, "
-                                     f"expected {expected[name]}")
-                th = t.detach().to(device=self.device, dtype=torch.float16).contiguous()
-                keep.append(th)
-                N.check(lib.sdw_clip_load_param(self._h, name.encode(), N.ptr(th), C.c_int64(th.numel()), N.stream_ptr()))
-            torch.cuda.current_stream().synchronize()
-        first = C.c_char_p()
-        missing = lib.sdw_clip_missing_params(self._h, C.byref(first))
-        if missing:
-            raise N.SdwError(f"{missing} CLIP parameters not loaded (first: {first.value.decode()})")
+        # position_ids is a buffer, not a parameter
+        self._model.load({k: v for k, v in sd.items() if not k.endswith("position_ids")}, strict)
 
     def to(self, device):
         if torch.device(device).type != "cuda":

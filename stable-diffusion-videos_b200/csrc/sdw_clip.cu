@@ -12,7 +12,6 @@
 
 #include <cmath>
 #include <cstring>
-#include <map>
 #include <string>
 #include <vector>
 
@@ -108,14 +107,6 @@ __global__ void clip_act_kernel(__half* __restrict__ x, int64_t n, int gelu_erf)
 // ---------------------------------------------------------------------------------------------
 // engine
 // ---------------------------------------------------------------------------------------------
-struct ClipParam {
-  void* dst = nullptr;   // packed fp16 weight / fp32 vector / raw fp16 table
-  int64_t numel = 0;
-  int kind = 0;          // 0: fp32 vector, 1: linear weight [N][K] -> pack_weight at row offset, 2: raw fp16 copy
-  int N = 0, K = 0;
-  bool loaded = false;
-};
-
 struct ClipLayer {
   float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bo, *b1, *b2;
   __half *wqkv, *wo, *w1, *w2;
@@ -123,70 +114,58 @@ struct ClipLayer {
 
 struct ClipEngine {
   sdw_clip_config cfg;
-  bool dry = true;
-  uint8_t* base = nullptr;
-  size_t used = 0, cap = 0;
-  std::map<std::string, ClipParam> params;
-  std::vector<std::string> order;
+  Arena arena{256};
+  size_t cap = 0;
+  ParamTable params;
   std::vector<ClipLayer> layers;
   __half *tok = nullptr, *pos = nullptr;
   float *lnf_g = nullptr, *lnf_b = nullptr;
   __half *x0 = nullptr, *x1 = nullptr, *h = nullptr, *qkv = nullptr, *ff = nullptr;
   int32_t* ids = nullptr;
 
-  template <typename T>
-  T* take(size_t n) {
-    used = (used + 255) & ~size_t(255);
-    T* p = dry ? nullptr : reinterpret_cast<T*>(base + used);
-    used += n * sizeof(T);
-    return p;
-  }
-  void reg(const std::string& name, void* dst, int64_t numel, int kind, int N = 0, int K = 0) {
-    ClipParam p;
-    p.dst = dst; p.numel = numel; p.kind = kind; p.N = N; p.K = K;
-    if (!params.count(name)) order.push_back(name);
-    params[name] = p;
-  }
-  void layout() {
+  void layout(void* base) {
     const sdw_clip_config& c = cfg;
     const int H = c.hidden, I = c.intermediate;
-    used = 0;
-    params.clear();
-    order.clear();
+    arena.reset(base);
+    params.clear(base != nullptr);
     layers.assign(c.layers, ClipLayer{});
-    tok = take<__half>(static_cast<size_t>(c.vocab) * H);
-    pos = take<__half>(static_cast<size_t>(c.max_positions) * H);
-    reg("text_model.embeddings.token_embedding.weight", tok, static_cast<int64_t>(c.vocab) * H, 2);
-    reg("text_model.embeddings.position_embedding.weight", pos, static_cast<int64_t>(c.max_positions) * H, 2);
+    tok = arena.take<__half>(static_cast<size_t>(c.vocab) * H);
+    pos = arena.take<__half>(static_cast<size_t>(c.max_positions) * H);
+    params.add("text_model.embeddings.token_embedding.weight", RAW, tok, static_cast<int64_t>(c.vocab) * H);
+    params.add("text_model.embeddings.position_embedding.weight", RAW, pos, static_cast<int64_t>(c.max_positions) * H);
     for (int i = 0; i < c.layers; ++i) {
       ClipLayer& L = layers[i];
       const std::string p = "text_model.encoder.layers." + std::to_string(i) + ".";
-      L.ln1_g = take<float>(H); L.ln1_b = take<float>(H); L.ln2_g = take<float>(H); L.ln2_b = take<float>(H);
-      L.bqkv = take<float>(3 * H); L.bo = take<float>(H); L.b1 = take<float>(I); L.b2 = take<float>(H);
-      L.wqkv = take<__half>(static_cast<size_t>(3) * H * H);
-      L.wo = take<__half>(static_cast<size_t>(H) * H);
-      L.w1 = take<__half>(static_cast<size_t>(I) * H);
-      L.w2 = take<__half>(static_cast<size_t>(H) * I);
-      reg(p + "layer_norm1.weight", L.ln1_g, H, 0); reg(p + "layer_norm1.bias", L.ln1_b, H, 0);
-      reg(p + "layer_norm2.weight", L.ln2_g, H, 0); reg(p + "layer_norm2.bias", L.ln2_b, H, 0);
+      L.ln1_g = arena.take<float>(H); L.ln1_b = arena.take<float>(H);
+      L.ln2_g = arena.take<float>(H); L.ln2_b = arena.take<float>(H);
+      L.bqkv = arena.take<float>(3 * H); L.bo = arena.take<float>(H);
+      L.b1 = arena.take<float>(I); L.b2 = arena.take<float>(H);
+      L.wqkv = arena.take<__half>(static_cast<size_t>(3) * H * H);
+      L.wo = arena.take<__half>(static_cast<size_t>(H) * H);
+      L.w1 = arena.take<__half>(static_cast<size_t>(I) * H);
+      L.w2 = arena.take<__half>(static_cast<size_t>(H) * I);
+      params.add(p + "layer_norm1.weight", VEC, L.ln1_g, H); params.add(p + "layer_norm1.bias", VEC, L.ln1_b, H);
+      params.add(p + "layer_norm2.weight", VEC, L.ln2_g, H); params.add(p + "layer_norm2.bias", VEC, L.ln2_b, H);
       const char* qkvn[3] = {"q_proj", "k_proj", "v_proj"};
       for (int k = 0; k < 3; ++k) {
-        reg(p + "self_attn." + qkvn[k] + ".weight", dry ? nullptr : L.wqkv + static_cast<size_t>(k) * H * H,
-            static_cast<int64_t>(H) * H, 1, H, H);
-        reg(p + "self_attn." + qkvn[k] + ".bias", dry ? nullptr : L.bqkv + k * H, H, 0);
+        params.add(p + "self_attn." + qkvn[k] + ".weight", PACKED, L.wqkv ? L.wqkv + static_cast<size_t>(k) * H * H : nullptr,
+                   static_cast<int64_t>(H) * H, H, H);
+        params.add(p + "self_attn." + qkvn[k] + ".bias", VEC, L.bqkv ? L.bqkv + k * H : nullptr, H);
       }
-      reg(p + "self_attn.out_proj.weight", L.wo, static_cast<int64_t>(H) * H, 1, H, H);
-      reg(p + "self_attn.out_proj.bias", L.bo, H, 0);
-      reg(p + "mlp.fc1.weight", L.w1, static_cast<int64_t>(I) * H, 1, I, H); reg(p + "mlp.fc1.bias", L.b1, I, 0);
-      reg(p + "mlp.fc2.weight", L.w2, static_cast<int64_t>(H) * I, 1, H, I); reg(p + "mlp.fc2.bias", L.b2, H, 0);
+      params.add(p + "self_attn.out_proj.weight", PACKED, L.wo, static_cast<int64_t>(H) * H, H, H);
+      params.add(p + "self_attn.out_proj.bias", VEC, L.bo, H);
+      params.add(p + "mlp.fc1.weight", PACKED, L.w1, static_cast<int64_t>(I) * H, I, H);
+      params.add(p + "mlp.fc1.bias", VEC, L.b1, I);
+      params.add(p + "mlp.fc2.weight", PACKED, L.w2, static_cast<int64_t>(H) * I, H, I);
+      params.add(p + "mlp.fc2.bias", VEC, L.b2, H);
     }
-    lnf_g = take<float>(H); lnf_b = take<float>(H);
-    reg("text_model.final_layer_norm.weight", lnf_g, H, 0);
-    reg("text_model.final_layer_norm.bias", lnf_b, H, 0);
+    lnf_g = arena.take<float>(H); lnf_b = arena.take<float>(H);
+    params.add("text_model.final_layer_norm.weight", VEC, lnf_g, H);
+    params.add("text_model.final_layer_norm.bias", VEC, lnf_b, H);
     const size_t T = static_cast<size_t>(c.max_batch) * c.max_positions;
-    x0 = take<__half>(T * H); x1 = take<__half>(T * H); h = take<__half>(T * H);
-    qkv = take<__half>(T * 3 * H); ff = take<__half>(T * I);
-    ids = take<int32_t>(T);
+    x0 = arena.take<__half>(T * H); x1 = arena.take<__half>(T * H); h = arena.take<__half>(T * H);
+    qkv = arena.take<__half>(T * 3 * H); ff = arena.take<__half>(T * I);
+    ids = arena.take<int32_t>(T);
   }
 };
 
@@ -214,9 +193,8 @@ int sdw_clip_create(const sdw_clip_config* cfg, sdw_clip** out) {
   SDW_REQUIRE(cfg->max_batch >= 1, "max_batch");
   ClipEngine* E = new ClipEngine();
   E->cfg = *cfg;
-  E->dry = true;
-  E->layout();
-  E->cap = E->used;
+  E->layout(nullptr);
+  E->cap = E->arena.off;
   *out = reinterpret_cast<sdw_clip*>(E);
   return 0;
 }
@@ -235,63 +213,32 @@ int sdw_clip_bind(sdw_clip* e, void* arena, uint64_t bytes) {
   SDW_REQUIRE(E && arena, "null");
   SDW_REQUIRE(bytes >= E->cap + 256, "arena too small");
   SDW_REQUIRE((reinterpret_cast<uintptr_t>(arena) & 255) == 0, "arena must be 256-byte aligned");
-  E->base = static_cast<uint8_t*>(arena);
-  E->dry = false;
-  E->layout();
+  E->layout(arena);
   return 0;
 }
 
-int sdw_clip_num_params(const sdw_clip* e) {
-  const ClipEngine* E = reinterpret_cast<const ClipEngine*>(e);
-  return E ? static_cast<int>(E->order.size()) : 0;
-}
+int sdw_clip_num_params(const sdw_clip* e) { return e ? reinterpret_cast<const ClipEngine*>(e)->params.size() : 0; }
 
 int sdw_clip_param_info(const sdw_clip* e, int index, const char** name, int64_t* numel) {
-  const ClipEngine* E = reinterpret_cast<const ClipEngine*>(e);
-  SDW_REQUIRE(E && index >= 0 && index < static_cast<int>(E->order.size()), "bad index");
-  if (name) *name = E->order[index].c_str();
-  if (numel) *numel = E->params.at(E->order[index]).numel;
-  return 0;
+  SDW_REQUIRE(e, "null");
+  return reinterpret_cast<const ClipEngine*>(e)->params.info(index, name, numel);
 }
 
 int sdw_clip_load_param(sdw_clip* e, const char* name, const void* data_f16, int64_t numel, void* stream) {
-  ClipEngine* E = reinterpret_cast<ClipEngine*>(e);
-  SDW_REQUIRE(E && name && data_f16 && !E->dry, "null / engine not bound");
-  auto it = E->params.find(name);
-  SDW_REQUIRE(it != E->params.end(), "unknown CLIP parameter");
-  ClipParam& p = it->second;
-  SDW_REQUIRE(numel == p.numel, "CLIP parameter size mismatch");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (p.kind == 0) {
-    if (int rc = half_to_float(static_cast<const __half*>(data_f16), static_cast<float*>(p.dst), numel, 0, st)) return rc;
-  } else if (p.kind == 1) {
-    if (int rc = pack_weight(data_f16, p.N, p.K, 1, 1, 0, p.dst, st)) return rc;
-  } else {
-    SDW_CUDA_OK(cudaMemcpyAsync(p.dst, data_f16, static_cast<size_t>(numel) * 2, cudaMemcpyDeviceToDevice, st));
-  }
-  p.loaded = true;
-  return 0;
+  SDW_REQUIRE(e, "null");
+  return reinterpret_cast<ClipEngine*>(e)->params.load(name, data_f16, numel, static_cast<cudaStream_t>(stream));
 }
 
 int sdw_clip_missing_params(const sdw_clip* e, const char** first_missing) {
-  const ClipEngine* E = reinterpret_cast<const ClipEngine*>(e);
-  if (!E) return -1;
-  int n = 0;
-  for (auto& name : E->order)
-    if (!E->params.at(name).loaded) {
-      if (n == 0 && first_missing) *first_missing = name.c_str();
-      ++n;
-    }
-  return n;
+  return e ? reinterpret_cast<const ClipEngine*>(e)->params.missing(first_missing) : -1;
 }
 
 int sdw_clip_forward(sdw_clip* e, const int32_t* ids, int B, void* out_f16, void* stream) {
   ClipEngine* E = reinterpret_cast<ClipEngine*>(e);
-  SDW_REQUIRE(E && ids && out_f16 && !E->dry, "null / engine not bound");
+  SDW_REQUIRE(E && ids && out_f16 && E->params.bound, "null / engine not bound");
   const sdw_clip_config& c = E->cfg;
   SDW_REQUIRE(B >= 1 && B <= c.max_batch, "batch exceeds max_batch");
-  const char* missing = nullptr;
-  SDW_REQUIRE(sdw_clip_missing_params(e, &missing) == 0, "CLIP parameters not loaded");
+  SDW_REQUIRE(E->params.missing(nullptr) == 0, "CLIP parameters not loaded");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int P = c.max_positions, H = c.hidden, I = c.intermediate;
   const int64_t T = static_cast<int64_t>(B) * P;

@@ -18,7 +18,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <functional>
-#include <map>
 #include <memory>
 #include <vector>
 
@@ -36,28 +35,13 @@ struct T {  // NHWC fp16 view
   int64_t pixels() const { return static_cast<int64_t>(B) * H * W; }
 };
 
-enum ParamKind { P_PACKED, P_RAW, P_VEC, P_PACKED_UP4 };
-struct ParamSlot {
-  ParamKind kind;
-  void* dst;
-  int N, C, kh, kw;
-  int geglu;
-  int64_t numel;
-  bool loaded = false;
-};
-
-using OpFn = std::function<int(cudaStream_t, int /*step*/)>;
-
 struct Engine {
   sdw_engine_config cfg{};
   bool dry = true;
-  uint8_t* base = nullptr;
-  size_t off = 0;
+  Arena arena{1024};
   size_t arena_bytes = 0;
-  std::map<std::string, ParamSlot> params;
-  std::vector<OpFn> prologue, unet_ops, vae_ops;
-  int n_launch_prologue = 0, n_launch_unet = 0, n_launch_vae = 0;
-  int* launch_counter = nullptr;
+  ParamTable params;
+  OpList prologue, unet_ops, vae_ops;
   // fixed buffers
   int Bn = 0;  // UNet batch = F * (guidance ? 2 : 1)
   __half* model_in = nullptr;   // [Bn][H][W][4]
@@ -88,22 +72,13 @@ struct Engine {
   int n_steps = 0;
   std::vector<sdw_step_coef> coefs;
   float init_sigma = 1.f, first_in_scale = 1.f;
-  // graph
-  cudaGraphExec_t graph_exec = nullptr;
-  int graph_steps = -1;
-  std::string err;
+  GraphCache graph;  // keyed by n_steps
 
   // ---- arena ---------------------------------------------------------------
-  void* alloc(size_t bytes, size_t align = 1024) {
-    off = (off + align - 1) / align * align;
-    void* p = dry ? nullptr : base + off;
-    off += bytes;
-    return p;
-  }
   T act(int B, int H, int W, int C) {
     T t;
     t.B = B; t.H = H; t.W = W; t.C = C; t.ld = C;
-    t.p = static_cast<__half*>(alloc(static_cast<size_t>(B) * H * W * C * 2));
+    t.p = static_cast<__half*>(arena.take(static_cast<size_t>(B) * H * W * C * 2));
     return t;
   }
   // ---- activation liveness.  The launch plan is a fixed sequence on one stream, so lifetimes are known at build time:
@@ -112,21 +87,14 @@ struct Engine {
   //   * the VAE decoder is a pure chain, its block outputs alternate between two PING-PONG slots;
   //   * weights, tables, skip-concat buffers, UNet block outputs and I/O stay in the persistent bump region.
   // Layout: [persistent | ping | pong | scratch]; the dry run measures the four sizes, the bound run places the bases.
-  size_t soff = 0, speak = 0, pers_bytes = 0, pp_peak[2] = {0, 0};
+  Arena scratch{1024};
+  size_t pers_bytes = 0, pp_peak[2] = {0, 0};
   int pp_count = 0;
-  uint8_t* sbase = nullptr;
   uint8_t* pp_base[2] = {nullptr, nullptr};
-  void* salloc(size_t bytes, size_t align = 1024) {
-    soff = (soff + align - 1) / align * align;
-    void* p = dry ? nullptr : sbase + soff;
-    soff += bytes;
-    speak = std::max(speak, soff);
-    return p;
-  }
   T tmp(int B, int H, int W, int C) {
     T t;
     t.B = B; t.H = H; t.W = W; t.C = C; t.ld = C;
-    t.p = static_cast<__half*>(salloc(static_cast<size_t>(B) * H * W * C * 2));
+    t.p = static_cast<__half*>(scratch.take(static_cast<size_t>(B) * H * W * C * 2));
     return t;
   }
   T pingpong(int B, int H, int W, int C) {  // the tensor allocated two calls ago is dead by construction (pure chain)
@@ -141,8 +109,8 @@ struct Engine {
   struct Scope {
     Engine* e;
     size_t mark;
-    explicit Scope(Engine* eng) : e(eng), mark(eng->soff) {}
-    ~Scope() { e->soff = mark; }
+    explicit Scope(Engine* eng) : e(eng), mark(eng->scratch.off) {}
+    ~Scope() { e->scratch.off = mark; }
   };
   static T slice(const T& big, int c0, int C) {
     T t = big;
@@ -156,47 +124,42 @@ struct Engine {
                          bool placed = false) {
     const int cp = (C + 63) / 64 * 64;
     const size_t bytes = static_cast<size_t>(N) * k * k * cp * 2;
-    __half* dst = placed ? into : static_cast<__half*>(alloc(bytes));
-    ParamSlot s{P_PACKED, dst, N, C, k, k, geglu, static_cast<int64_t>(N) * C * k * k};
-    params[name] = s;
+    __half* dst = placed ? into : static_cast<__half*>(arena.take(bytes));
+    params.add(name, PACKED, dst, static_cast<int64_t>(N) * C * k * k, N, C, k, k, geglu);
     return dst;
   }
   // upsampler conv: four parity blocks of pre-summed 2x2 taps (pack_weight_up4)
   const __half* w_packed_up4(const std::string& name, int N, int C) {
     const int cp = (C + 63) / 64 * 64;
-    __half* dst = static_cast<__half*>(alloc(static_cast<size_t>(N) * 16 * cp * 2));
-    params[name] = ParamSlot{P_PACKED_UP4, dst, N, C, 3, 3, 0, static_cast<int64_t>(N) * C * 9};
+    __half* dst = static_cast<__half*>(arena.take(static_cast<size_t>(N) * 16 * cp * 2));
+    params.add(name, PACKED_UP4, dst, static_cast<int64_t>(N) * C * 9, N, C, 3, 3);
     return dst;
   }
   const __half* w_raw(const std::string& name, int64_t numel) {
-    __half* dst = static_cast<__half*>(alloc(static_cast<size_t>(numel) * 2));
-    params[name] = ParamSlot{P_RAW, dst, 0, 0, 0, 0, 0, numel};
+    __half* dst = static_cast<__half*>(arena.take(static_cast<size_t>(numel) * 2));
+    params.add(name, RAW, dst, numel);
     return dst;
   }
   const float* vec(const std::string& name, int n, int geglu_N = 0) {
-    float* dst = static_cast<float*>(alloc(static_cast<size_t>(n) * 4));
-    params[name] = ParamSlot{P_VEC, dst, geglu_N, 0, 0, 0, 0, n};
+    float* dst = static_cast<float*>(arena.take(static_cast<size_t>(n) * 4));
+    params.add(name, VEC, dst, n, geglu_N, 0, 1, 1, geglu_N > 0);
     return dst;
   }
 
   // ---- op emission ---------------------------------------------------------
-  std::vector<OpFn>* cur = nullptr;
-  int* cur_count = nullptr;
-  // tags parallel to the op lists (tooling: sdw_engine_debug_profile); `tag_next` names the op about to be emitted
-  std::vector<std::string> prologue_tags, unet_tags, vae_tags;
-  std::string tag_next;
+  OpList* cur = nullptr;
+  std::string tag_next;  // names the op about to be emitted (tooling: sdw_engine_debug_profile)
   void emit(OpFn f, int launches = 1) {
     if (!dry) {
-      cur->push_back(std::move(f));
-      std::vector<std::string>& tags = cur == &prologue ? prologue_tags : (cur == &unet_ops ? unet_tags : vae_tags);
-      tags.push_back(tag_next.empty() ? std::string("op") : tag_next);
+      cur->ops.push_back(std::move(f));
+      cur->tags.push_back(tag_next.empty() ? std::string("op") : tag_next);
     }
     tag_next.clear();
-    *cur_count += launches;
+    cur->launches += launches;
   }
   int emit_gemm(const GemmDesc& d, const float* rowvec_table = nullptr, int rowvec_stride = 0) {
     if (dry) {
-      *cur_count += 1;
+      cur->launches += 1;
       return 0;
     }
     auto L = std::make_shared<GemmLaunch>();
@@ -215,8 +178,7 @@ struct Engine {
         return launch_gemm(l, st);
       }
       return launch_gemm(*L, st);
-    }, 0);
-    *cur_count += 1;
+    });
     return 0;
   }
   // tiled = True: circular padding (reference P:841-858 patches every Conv2d to padding_mode="circular").  A 3x3 conv on the
@@ -267,8 +229,8 @@ struct Engine {
     Scope scope(this);
     T xp = tmp(n.B, n.H + 2, n.W + 2, n.C);
     const size_t pp = static_cast<size_t>(n.B) * (n.H + 2) * (n.W + 2);
-    float* f32p = static_cast<float*>(salloc(pp * oc * 4));
-    uint8_t* u8p = out_u8 ? static_cast<uint8_t*>(salloc(pp * oc)) : nullptr;
+    float* f32p = static_cast<float*>(scratch.take(pp * oc * 4));
+    uint8_t* u8p = out_u8 ? static_cast<uint8_t*>(scratch.take(pp * oc)) : nullptr;
     emit([=](cudaStream_t st, int) {
       if (int e = wrap_pad(n.p, n.ld * 2, n.B, n.H, n.W, n.C * 2, 1, xp.p, st)) return e;
       if (int e = conv_out_small(xp.p, xp.ld, xp.B, xp.H, xp.W, xp.C, w, b, oc, f32p, u8p, st)) return e;
@@ -332,7 +294,7 @@ struct Engine {
                 int Nq, int Nk, int heads, int d, const T& out) {
     if (use_flash && attn_supported(d)) {
       if (dry) {
-        *cur_count += 1;
+        cur->launches += 1;
         return 0;
       }
       AttnDesc a;
@@ -395,7 +357,7 @@ struct Engine {
       TProj tp;
       tp.w = w_raw(pre + ".time_emb_proj.weight", static_cast<int64_t>(cout) * temb_ch());
       tp.b = vec(pre + ".time_emb_proj.bias", cout);
-      tp.table = static_cast<float*>(alloc(static_cast<size_t>(cfg.max_steps) * cout * 4));
+      tp.table = static_cast<float*>(arena.take(static_cast<size_t>(cfg.max_steps) * cout * 4));
       tp.cout = cout;
       tprojs.push_back(tp);
       table = tp.table;
@@ -430,14 +392,14 @@ struct Engine {
     T t1 = tmp(x.B, x.H, x.W, C);
     // --- self attention
     ln(hA, tb + ".norm1", t1);
-    __half* wqkv = static_cast<__half*>(alloc(static_cast<size_t>(3) * C * ((C + 63) / 64 * 64) * 2));
+    __half* wqkv = static_cast<__half*>(arena.take(static_cast<size_t>(3) * C * ((C + 63) / 64 * 64) * 2));
     const int cp = (C + 63) / 64 * 64;
     w_packed(tb + ".attn1.to_q.weight", C, C, 1, 0, wqkv, true);
     w_packed(tb + ".attn1.to_k.weight", C, C, 1, 0, wqkv ? wqkv + static_cast<size_t>(C) * cp : nullptr, true);
     w_packed(tb + ".attn1.to_v.weight", C, C, 1, 0, wqkv ? wqkv + static_cast<size_t>(2) * C * cp : nullptr, true);
     T qk = tmp(x.B, x.H, x.W, 2 * C);
     const int64_t vt_ld = (Nq + 7) / 8 * 8;
-    __half* vt = static_cast<__half*>(salloc(static_cast<size_t>(Bq) * heads * d * vt_ld * 2));
+    __half* vt = static_cast<__half*>(scratch.take(static_cast<size_t>(Bq) * heads * d * vt_ld * 2));
     {
       GemmDesc g;
       g.A = t1.p; g.C = C; g.W = Nq; g.H = 1; g.B = Bq;
@@ -459,17 +421,15 @@ struct Engine {
     T q2 = tmp(x.B, x.H, x.W, C);
     if (int e = linear(t1, w_packed(tb + ".attn2.to_q.weight", C, C, 1), nullptr, C, q2)) return e;
     const int dcp = (D + 63) / 64 * 64;
-    __half* wkv = static_cast<__half*>(alloc(static_cast<size_t>(2) * C * dcp * 2));
+    __half* wkv = static_cast<__half*>(arena.take(static_cast<size_t>(2) * C * dcp * 2));
     w_packed(tb + ".attn2.to_k.weight", C, D, 1, 0, wkv, true);
     w_packed(tb + ".attn2.to_v.weight", C, D, 1, 0, wkv ? wkv + static_cast<size_t>(C) * dcp : nullptr, true);
-    __half* kx = static_cast<__half*>(alloc(static_cast<size_t>(Bq) * tokens * C * 2));
+    __half* kx = static_cast<__half*>(arena.take(static_cast<size_t>(Bq) * tokens * C * 2));
     const int64_t vx_ld = (tokens + 7) / 8 * 8;
-    __half* vx = static_cast<__half*>(alloc(static_cast<size_t>(Bq) * heads * d * vx_ld * 2));
+    __half* vx = static_cast<__half*>(arena.take(static_cast<size_t>(Bq) * heads * d * vx_ld * 2));
     {
-      std::vector<OpFn>* save = cur;
-      int* save_c = cur_count;
+      OpList* save = cur;
       cur = &prologue;
-      cur_count = &n_launch_prologue;
       GemmDesc g;
       g.A = ctx; g.C = D; g.W = Bq * tokens; g.H = 1; g.B = 1;
       g.sW = D;
@@ -479,7 +439,6 @@ struct Engine {
       g.vt_col0 = C; g.vt_d = d; g.vt_heads = heads; g.vt_ntok = tokens; g.vt = vx; g.vt_ld = vx_ld;
       int e = emit_gemm(g);
       cur = save;
-      cur_count = save_c;
       if (e) return e;
     }
     if (int e = attention(q2.p, q2.ld, kx, C, vx, vx_ld, Bq, Nq, tokens, heads, d, ao)) return e;
@@ -504,7 +463,6 @@ struct Engine {
 
   int build_unet() {
     cur = &unet_ops;
-    cur_count = &n_launch_unet;
     cfg_groups = cfg.norm_num_groups;
     const int nlev = cfg.num_levels, L = cfg.layers_per_block;
     const int* ch = cfg.block_out_channels;
@@ -636,7 +594,6 @@ struct Engine {
 
   int build_vae() {
     cur = &vae_ops;
-    cur_count = &n_launch_vae;
     cfg_groups = cfg.vae_norm_num_groups;
     const int F = cfg.frames, H0 = cfg.latent_h, W0 = cfg.latent_w, lc = cfg.in_channels;
     const int nlev = cfg.vae_num_levels;
@@ -670,17 +627,17 @@ struct Engine {
       T g0 = tmp(F, H0, W0, ctop);
       gn(a, ap + ".group_norm", 1e-6f, 0, g0);
       const int C = ctop, Nq = H0 * W0, cp = (C + 63) / 64 * 64;
-      __half* wqkv = static_cast<__half*>(alloc(static_cast<size_t>(3) * C * cp * 2));
+      __half* wqkv = static_cast<__half*>(arena.take(static_cast<size_t>(3) * C * cp * 2));
       w_packed(ap + ".to_q.weight", C, C, 1, 0, wqkv, true);
       w_packed(ap + ".to_k.weight", C, C, 1, 0, wqkv ? wqkv + static_cast<size_t>(C) * cp : nullptr, true);
       w_packed(ap + ".to_v.weight", C, C, 1, 0, wqkv ? wqkv + static_cast<size_t>(2) * C * cp : nullptr, true);
-      float* bqkv = static_cast<float*>(alloc(static_cast<size_t>(3) * C * 4));
-      params[ap + ".to_q.bias"] = ParamSlot{P_VEC, bqkv, 0, 0, 0, 0, 0, C};
-      params[ap + ".to_k.bias"] = ParamSlot{P_VEC, bqkv ? bqkv + C : nullptr, 0, 0, 0, 0, 0, C};
-      params[ap + ".to_v.bias"] = ParamSlot{P_VEC, bqkv ? bqkv + 2 * C : nullptr, 0, 0, 0, 0, 0, C};
+      float* bqkv = static_cast<float*>(arena.take(static_cast<size_t>(3) * C * 4));
+      params.add(ap + ".to_q.bias", VEC, bqkv, C);
+      params.add(ap + ".to_k.bias", VEC, bqkv ? bqkv + C : nullptr, C);
+      params.add(ap + ".to_v.bias", VEC, bqkv ? bqkv + 2 * C : nullptr, C);
       T qk = tmp(F, H0, W0, 2 * C);
       const int64_t vt_ld = (Nq + 7) / 8 * 8;
-      __half* vt = static_cast<__half*>(salloc(static_cast<size_t>(F) * C * vt_ld * 2));
+      __half* vt = static_cast<__half*>(scratch.take(static_cast<size_t>(F) * C * vt_ld * 2));
       {
         GemmDesc g;
         g.A = g0.p; g.C = C; g.W = Nq; g.H = 1; g.B = F;
@@ -732,39 +689,37 @@ struct Engine {
     return 0;
   }
 
-  int build(bool dry_run, void* arena) {
+  int build(bool dry_run, void* base) {
     dry = dry_run;
-    base = static_cast<uint8_t*>(arena);
-    off = 0;
-    soff = 0;
+    arena.reset(base);
     pp_count = 0;
     if (dry) {
-      speak = pp_peak[0] = pp_peak[1] = 0;
+      pp_peak[0] = pp_peak[1] = 0;
+      scratch.reset(nullptr);
     } else {  // sizes measured by the dry run
-      pp_base[0] = base + pers_bytes;
+      pp_base[0] = static_cast<uint8_t*>(base) + pers_bytes;
       pp_base[1] = pp_base[0] + (pp_peak[0] + 1023) / 1024 * 1024;
-      sbase = pp_base[1] + (pp_peak[1] + 1023) / 1024 * 1024;
+      scratch.reset(pp_base[1] + (pp_peak[1] + 1023) / 1024 * 1024);
     }
-    params.clear();
+    params.clear(!dry);
     prologue.clear(); unet_ops.clear(); vae_ops.clear(); tprojs.clear();
-    n_launch_prologue = n_launch_unet = n_launch_vae = 0;
     const int F = cfg.frames, H = cfg.latent_h, W = cfg.latent_w, lc = cfg.in_channels;
     Bn = F * (cfg.guidance ? 2 : 1);
     const int64_t nlat = static_cast<int64_t>(F) * lc * H * W;
-    model_in = static_cast<__half*>(alloc(static_cast<size_t>(Bn) * H * W * lc * 2));
-    eps = static_cast<float*>(alloc(static_cast<size_t>(Bn) * H * W * cfg.out_channels * 4));
-    x = static_cast<float*>(alloc(nlat * 4));
-    x_base = static_cast<float*>(alloc(nlat * 4));
-    hist = static_cast<float*>(alloc(nlat * 4 * 4));
-    lat_stage = alloc(nlat * 4);
+    model_in = static_cast<__half*>(arena.take(static_cast<size_t>(Bn) * H * W * lc * 2));
+    eps = static_cast<float*>(arena.take(static_cast<size_t>(Bn) * H * W * cfg.out_channels * 4));
+    x = static_cast<float*>(arena.take(nlat * 4));
+    x_base = static_cast<float*>(arena.take(nlat * 4));
+    hist = static_cast<float*>(arena.take(nlat * 4 * 4));
+    lat_stage = arena.take(nlat * 4);
     const int64_t per = static_cast<int64_t>(cfg.ctx_tokens) * cfg.cross_attention_dim;
-    ctx = static_cast<__half*>(alloc(static_cast<size_t>(Bn) * per * 2));
-    cond_stage = static_cast<__half*>(alloc(static_cast<size_t>(Bn) * per * 2));  // room for a full [Bn] context
-    uncond_stage = static_cast<__half*>(alloc(static_cast<size_t>(cfg.frames) * per * 2));
+    ctx = static_cast<__half*>(arena.take(static_cast<size_t>(Bn) * per * 2));
+    cond_stage = static_cast<__half*>(arena.take(static_cast<size_t>(Bn) * per * 2));  // room for a full [Bn] context
+    uncond_stage = static_cast<__half*>(arena.take(static_cast<size_t>(cfg.frames) * per * 2));
     const int OH = H * cfg.vae_scale, OW = W * cfg.vae_scale;
-    out_u8 = static_cast<uint8_t*>(alloc(static_cast<size_t>(F) * OH * OW * cfg.vae_out_channels));
-    out_img_f32 = static_cast<float*>(alloc(static_cast<size_t>(F) * OH * OW * cfg.vae_out_channels * 4));
-    gn_ws = static_cast<float2*>(alloc(gn_workspace_bytes(std::max(Bn, F))));
+    out_u8 = static_cast<uint8_t*>(arena.take(static_cast<size_t>(F) * OH * OW * cfg.vae_out_channels));
+    out_img_f32 = static_cast<float*>(arena.take(static_cast<size_t>(F) * OH * OW * cfg.vae_out_channels * 4));
+    gn_ws = static_cast<float2*>(arena.take(gn_workspace_bytes(std::max(Bn, F))));
     // attention score scratch of the UNFUSED path: the VAE mid attention (d = 512), and UNet level-0 self attention only
     // when its head dim has no fused kernel (or SDW_NO_FLASH)
     {
@@ -780,17 +735,17 @@ struct Engine {
       const int64_t n0p = (n0 + 7) / 8 * 8;
       int64_t vae_s = static_cast<int64_t>(unfused_chunk(F, 1, n0, n0p)) * n0 * n0p;  // a chunk of samples, not the batch
       S_elems = static_cast<size_t>(std::max(unet_s, vae_s));
-      S = static_cast<__half*>(alloc(S_elems * 2));
+      S = static_cast<__half*>(arena.take(S_elems * 2));
     }
-    t_dev = static_cast<float*>(alloc(static_cast<size_t>(cfg.max_steps) * 4));
-    t_sin = static_cast<float*>(alloc(static_cast<size_t>(cfg.max_steps) * cfg.block_out_channels[0] * 4));
-    t_h1 = static_cast<float*>(alloc(static_cast<size_t>(cfg.max_steps) * temb_ch() * 4));
-    temb = static_cast<float*>(alloc(static_cast<size_t>(cfg.max_steps) * temb_ch() * 4));
+    t_dev = static_cast<float*>(arena.take(static_cast<size_t>(cfg.max_steps) * 4));
+    t_sin = static_cast<float*>(arena.take(static_cast<size_t>(cfg.max_steps) * cfg.block_out_channels[0] * 4));
+    t_h1 = static_cast<float*>(arena.take(static_cast<size_t>(cfg.max_steps) * temb_ch() * 4));
+    temb = static_cast<float*>(arena.take(static_cast<size_t>(cfg.max_steps) * temb_ch() * 4));
     if (int e = build_unet()) return e;
     if (int e = build_vae()) return e;
     if (dry) {
-      pers_bytes = (off + 4095) / 4096 * 4096;
-      arena_bytes = pers_bytes + (pp_peak[0] + 1023) / 1024 * 1024 + (pp_peak[1] + 1023) / 1024 * 1024 + speak + 4096;
+      pers_bytes = (arena.off + 4095) / 4096 * 4096;
+      arena_bytes = pers_bytes + (pp_peak[0] + 1023) / 1024 * 1024 + (pp_peak[1] + 1023) / 1024 * 1024 + scratch.peak + 4096;
     }
     return 0;
   }
@@ -866,10 +821,7 @@ int sdw_engine_create(const sdw_engine_config* cfg, sdw_engine** out) {
 }
 
 void sdw_engine_destroy(sdw_engine* e) {
-  Engine* E = reinterpret_cast<Engine*>(e);
-  if (!E) return;
-  if (E->graph_exec) cudaGraphExecDestroy(E->graph_exec);
-  delete E;
+  delete reinterpret_cast<Engine*>(e);
 }
 
 int sdw_engine_arena_bytes(const sdw_engine* e, uint64_t* bytes) {
@@ -884,61 +836,24 @@ int sdw_engine_bind(sdw_engine* e, void* arena, uint64_t bytes) {
   SDW_REQUIRE(bytes >= E->arena_bytes, "arena too small");
   SDW_REQUIRE(reinterpret_cast<uintptr_t>(arena) % 1024 == 0, "arena must be 1024-byte aligned");
   if (int err = gemm_init()) return err;
-  if (E->graph_exec) {
-    cudaGraphExecDestroy(E->graph_exec);
-    E->graph_exec = nullptr;
-  }
+  E->graph.reset();
   return E->build(false, arena);
 }
 
-int sdw_engine_num_params(const sdw_engine* e) { return e ? static_cast<int>(reinterpret_cast<const Engine*>(e)->params.size()) : -1; }
+int sdw_engine_num_params(const sdw_engine* e) { return e ? reinterpret_cast<const Engine*>(e)->params.size() : -1; }
 
 int sdw_engine_param_info(const sdw_engine* e, int index, const char** name, int64_t* numel) {
-  const Engine* E = reinterpret_cast<const Engine*>(e);
-  SDW_REQUIRE(E && index >= 0 && index < static_cast<int>(E->params.size()), "bad index");
-  auto it = E->params.begin();
-  std::advance(it, index);
-  if (name) *name = it->first.c_str();
-  if (numel) *numel = it->second.numel;
-  return 0;
+  SDW_REQUIRE(e, "null");
+  return reinterpret_cast<const Engine*>(e)->params.info(index, name, numel);
 }
 
 int sdw_engine_load_param(sdw_engine* e, const char* name, const void* src_f16, int64_t numel, void* stream) {
-  Engine* E = reinterpret_cast<Engine*>(e);
-  SDW_REQUIRE(E && name && src_f16, "null");
-  SDW_REQUIRE(!E->dry, "engine not bound to an arena");
-  auto it = E->params.find(name);
-  if (it == E->params.end()) {
-    set_error(std::string("unknown parameter: ") + name);
-    return 1;
-  }
-  ParamSlot& s = it->second;
-  if (s.numel != numel) {
-    set_error(std::string("parameter size mismatch for ") + name + ": expected " + std::to_string(s.numel) + ", got " +
-              std::to_string(numel));
-    return 1;
-  }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int rc = 0;
-  if (s.kind == P_PACKED) rc = pack_weight(src_f16, s.N, s.C, s.kh, s.kw, s.geglu, s.dst, st);
-  else if (s.kind == P_PACKED_UP4) rc = pack_weight_up4(src_f16, s.N, s.C, s.dst, st);
-  else if (s.kind == P_RAW) {
-    SDW_CUDA_OK(cudaMemcpyAsync(s.dst, src_f16, static_cast<size_t>(numel) * 2, cudaMemcpyDeviceToDevice, st));
-  } else rc = half_to_float(static_cast<const __half*>(src_f16), static_cast<float*>(s.dst), numel, s.N, st);
-  if (rc == 0) s.loaded = true;
-  return rc;
+  SDW_REQUIRE(e, "null");
+  return reinterpret_cast<Engine*>(e)->params.load(name, src_f16, numel, static_cast<cudaStream_t>(stream));
 }
 
 int sdw_engine_missing_params(const sdw_engine* e, const char** first_missing) {
-  const Engine* E = reinterpret_cast<const Engine*>(e);
-  SDW_REQUIRE(E, "null");
-  int n = 0;
-  for (auto& kv : E->params)
-    if (!kv.second.loaded) {
-      if (n == 0 && first_missing) *first_missing = kv.first.c_str();
-      ++n;
-    }
-  return n;
+  return e ? reinterpret_cast<const Engine*>(e)->params.missing(first_missing) : -1;
 }
 
 int sdw_engine_set_schedule(sdw_engine* e, int n_steps, const float* timesteps, const sdw_step_coef* coefs,
@@ -952,10 +867,7 @@ int sdw_engine_set_schedule(sdw_engine* e, int n_steps, const float* timesteps, 
   E->coefs.assign(coefs, coefs + n_steps);
   E->init_sigma = init_noise_sigma;
   E->first_in_scale = first_in_scale;
-  if (E->graph_exec) {
-    cudaGraphExecDestroy(E->graph_exec);
-    E->graph_exec = nullptr;
-  }
+  E->graph.reset();
   SDW_CUDA_OK(cudaMemcpyAsync(E->t_dev, timesteps, static_cast<size_t>(n_steps) * 4, cudaMemcpyHostToDevice, st));
   SDW_CUDA_OK(cudaStreamSynchronize(st));  // the host array may be a temporary
   const int c0 = E->cfg.block_out_channels[0], tc = E->temb_ch();
@@ -967,28 +879,22 @@ int sdw_engine_set_schedule(sdw_engine* e, int n_steps, const float* timesteps, 
   return 0;
 }
 
-static int run_ops(std::vector<OpFn>& ops, cudaStream_t st, int step) {
-  for (auto& f : ops)
-    if (int rc = f(st, step)) return rc;
-  return 0;
-}
-
 static int run_all(Engine* E, cudaStream_t st) {
   const sdw_engine_config& c = E->cfg;
   const int F = c.frames, H = c.latent_h, W = c.latent_w, lc = c.in_channels;
   const int64_t per = static_cast<int64_t>(c.ctx_tokens) * c.cross_attention_dim;
   if (int rc = unet_ctx_assemble(E->cond_stage, E->uncond_stage, F, c.guidance, per, E->ctx, st, E->uncond_batch > 1)) return rc;
-  if (int rc = run_ops(E->prologue, st, 0)) return rc;
+  if (int rc = E->prologue.run(st, 0)) return rc;
   if (int rc = latents_init(E->lat_stage, 0, E->init_sigma, E->first_in_scale, E->x, E->model_in, lc, c.guidance, F, lc,
                             H, W, st))
     return rc;
   for (int s = 0; s < E->n_steps; ++s) {
-    if (int rc = run_ops(E->unet_ops, st, s)) return rc;
+    if (int rc = E->unet_ops.run(st, s)) return rc;
     if (int rc = cfg_sched_step(E->eps, c.guidance, E->x, E->x_base, E->hist, &E->coefs[s], F, lc, H, W,
                                 s + 1 < E->n_steps ? E->model_in : nullptr, lc, st))
       return rc;
   }
-  return run_ops(E->vae_ops, st, 0);
+  return E->vae_ops.run(st, 0);
 }
 
 static int stage_inputs(Engine* E, const float* latents_f32, const void* cond_f16, const void* uncond_f16,
@@ -1023,25 +929,7 @@ int sdw_engine_sample(sdw_engine* e, const float* latents_f32, const void* cond_
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = stage_inputs(E, latents_f32, cond_f16, uncond_f16, st)) return rc;
   if (use_graph) {
-    if (!E->graph_exec || E->graph_steps != E->n_steps) {
-      if (E->graph_exec) {
-        cudaGraphExecDestroy(E->graph_exec);
-        E->graph_exec = nullptr;
-      }
-      cudaGraph_t graph = nullptr;
-      SDW_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      int rc = run_all(E, st);
-      cudaError_t ce = cudaStreamEndCapture(st, &graph);
-      if (rc) {
-        if (graph) cudaGraphDestroy(graph);
-        return rc;
-      }
-      SDW_CUDA_OK(ce);
-      SDW_CUDA_OK(cudaGraphInstantiate(&E->graph_exec, graph, 0));
-      cudaGraphDestroy(graph);
-      E->graph_steps = E->n_steps;
-    }
-    SDW_CUDA_OK(cudaGraphLaunch(E->graph_exec, st));
+    if (int rc = E->graph.launch(E->n_steps, st, [E](cudaStream_t s) { return run_all(E, s); })) return rc;
   } else {
     if (int rc = run_all(E, st)) return rc;
   }
@@ -1062,7 +950,7 @@ int sdw_engine_sample_begin(sdw_engine* e, const float* latents_f32, const void*
   if (int rc = stage_inputs(E, latents_f32, cond_f16, uncond_f16, st)) return rc;
   const int64_t per = static_cast<int64_t>(c.ctx_tokens) * c.cross_attention_dim;
   if (int rc = unet_ctx_assemble(E->cond_stage, E->uncond_stage, c.frames, c.guidance, per, E->ctx, st, E->uncond_batch > 1)) return rc;
-  if (int rc = run_ops(E->prologue, st, 0)) return rc;
+  if (int rc = E->prologue.run(st, 0)) return rc;
   return latents_init(E->lat_stage, 0, E->init_sigma, E->first_in_scale, E->x, E->model_in, c.in_channels, c.guidance,
                       c.frames, c.in_channels, c.latent_h, c.latent_w, st);
 }
@@ -1074,7 +962,7 @@ int sdw_engine_sample_steps(sdw_engine* e, int s0, int s1, float* out_latents, v
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const sdw_engine_config& c = E->cfg;
   for (int s = s0; s < s1; ++s) {
-    if (int rc = run_ops(E->unet_ops, st, s)) return rc;
+    if (int rc = E->unet_ops.run(st, s)) return rc;
     if (int rc = cfg_sched_step(E->eps, c.guidance, E->x, E->x_base, E->hist, &E->coefs[s], c.frames, c.in_channels,
                                 c.latent_h, c.latent_w, s + 1 < E->n_steps ? E->model_in : nullptr, c.in_channels, st))
       return rc;
@@ -1086,7 +974,7 @@ int sdw_engine_sample_end(sdw_engine* e, uint8_t* out_u8, float* out_latents, fl
   Engine* E = reinterpret_cast<Engine*>(e);
   SDW_REQUIRE(E && out_u8 && !E->dry, "null / engine not bound");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (int rc = run_ops(E->vae_ops, st, 0)) return rc;
+  if (int rc = E->vae_ops.run(st, 0)) return rc;
   return copy_outputs(E, out_u8, out_latents, out_raw_f32, st);
 }
 
@@ -1094,10 +982,7 @@ int sdw_engine_set_uncond_batch(sdw_engine* e, int n) {
   Engine* E = reinterpret_cast<Engine*>(e);
   SDW_REQUIRE(E && !E->dry, "engine not bound");
   SDW_REQUIRE(n == 1 || n == E->cfg.frames, "the unconditional batch is 1 (shared) or `frames` (one per frame)");
-  if (n != E->uncond_batch && E->graph_exec) {  // the captured graph has the other addressing baked in
-    cudaGraphExecDestroy(E->graph_exec);
-    E->graph_exec = nullptr;
-  }
+  if (n != E->uncond_batch) E->graph.reset();  // the captured graph has the other addressing baked in
   E->uncond_batch = n;
   return 0;
 }
@@ -1105,9 +990,9 @@ int sdw_engine_set_uncond_batch(sdw_engine* e, int n) {
 int sdw_engine_launches(const sdw_engine* e, int* prologue, int* unet, int* vae) {
   const Engine* E = reinterpret_cast<const Engine*>(e);
   SDW_REQUIRE(E, "null");
-  if (prologue) *prologue = E->n_launch_prologue + 1;
-  if (unet) *unet = E->n_launch_unet;
-  if (vae) *vae = E->n_launch_vae;
+  if (prologue) *prologue = E->prologue.launches + 1;
+  if (unet) *unet = E->unet_ops.launches;
+  if (vae) *vae = E->vae_ops.launches;
   return 0;
 }
 
@@ -1120,28 +1005,8 @@ int sdw_engine_debug_profile(sdw_engine* e, const char* path, void* stream) {
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   FILE* f = std::fopen(path, "w");
   SDW_REQUIRE(f, "cannot open the profile file");
-  struct Sec { const char* name; std::vector<OpFn>* ops; std::vector<std::string>* tags; };
-  Sec secs[2] = {{"unet", &E->unet_ops, &E->unet_tags}, {"vae", &E->vae_ops, &E->vae_tags}};
-  int rc = 0;
-  for (const Sec& sc : secs) {
-    if ((rc = run_ops(*sc.ops, st, 0))) break;
-    const size_t n = sc.ops->size();
-    std::vector<cudaEvent_t> ev(n + 1);
-    for (auto& x : ev) cudaEventCreate(&x);
-    cudaEventRecord(ev[0], st);
-    for (size_t i = 0; i < n && !rc; ++i) {
-      rc = (*sc.ops)[i](st, 0);
-      cudaEventRecord(ev[i + 1], st);
-    }
-    cudaStreamSynchronize(st);
-    for (size_t i = 0; i < n && !rc; ++i) {
-      float ms = 0.f;
-      cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-      std::fprintf(f, "%s\t%zu\t%.2f\t%s\n", sc.name, i, ms * 1e3f, (*sc.tags)[i].c_str());
-    }
-    for (auto& x : ev) cudaEventDestroy(x);
-    if (rc) break;
-  }
+  int rc = profile_ops(f, "unet", E->unet_ops, st, 0);
+  if (!rc) rc = profile_ops(f, "vae", E->vae_ops, st, 0);
   std::fclose(f);
   if (rc) return rc;
   SDW_CUDA_OK(cudaGetLastError());
@@ -1162,8 +1027,8 @@ int sdw_engine_debug_unet(sdw_engine* e, const float* x_nchw, int step, const vo
   if (int rc = latents_init(x_nchw, 0, 1.f, 1.f, E->hist, E->model_in, c.in_channels, 0, E->Bn, c.in_channels,
                             c.latent_h, c.latent_w, st))
     return rc;
-  if (int rc = run_ops(E->prologue, st, 0)) return rc;
-  if (int rc = run_ops(E->unet_ops, st, step)) return rc;
+  if (int rc = E->prologue.run(st, 0)) return rc;
+  if (int rc = E->unet_ops.run(st, step)) return rc;
   SDW_CUDA_OK(cudaMemcpyAsync(eps_nhwc_out, E->eps,
                               static_cast<size_t>(E->Bn) * c.latent_h * c.latent_w * c.out_channels * 4,
                               cudaMemcpyDeviceToDevice, st));
@@ -1189,7 +1054,7 @@ int sdw_engine_debug_vae(sdw_engine* e, const float* latents_nchw, uint8_t* out_
   const sdw_engine_config& c = E->cfg;
   const int64_t nlat = static_cast<int64_t>(c.frames) * c.in_channels * c.latent_h * c.latent_w;
   SDW_CUDA_OK(cudaMemcpyAsync(E->x, latents_nchw, nlat * 4, cudaMemcpyDeviceToDevice, st));
-  if (int rc = run_ops(E->vae_ops, st, 0)) return rc;
+  if (int rc = E->vae_ops.run(st, 0)) return rc;
   const size_t n = static_cast<size_t>(c.frames) * c.latent_h * c.vae_scale * c.latent_w * c.vae_scale * c.vae_out_channels;
   SDW_CUDA_OK(cudaMemcpyAsync(out_u8, E->out_u8, n, cudaMemcpyDeviceToDevice, st));
   if (out_f32_nhwc) SDW_CUDA_OK(cudaMemcpyAsync(out_f32_nhwc, E->out_img_f32, n * 4, cudaMemcpyDeviceToDevice, st));

@@ -28,7 +28,7 @@
 #include <algorithm>
 #include <cstdio>
 #include <functional>
-#include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -36,23 +36,7 @@
 
 namespace sdw {
 
-__global__ void esr_bias_kernel(const __half* __restrict__ in, float* __restrict__ out, int n, float scale) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = __half2float(in[i]) * scale;
-}
-
 namespace {
-
-enum EsrKind : int { K_BIAS = 0, K_CONV3 = 1, K_UP4 = 2, K_RAW = 3 };
-
-struct EsrParam {
-  void* dst = nullptr;
-  int64_t numel = 0;
-  int kind = 0;
-  int N = 0, C = 0;
-  float scale = 1.f;  // biases of conv5: 0.2 (rdb1, rdb2) or 0.04 (rdb3)
-  bool loaded = false;
-};
 
 struct EsrConv {
   __half* w = nullptr;
@@ -61,64 +45,47 @@ struct EsrConv {
 
 struct EsrEngine {
   sdw_upsampler_config cfg;
-  bool dry = true;
-  uint8_t* base = nullptr;
-  size_t used = 0, cap = 0;
-  std::map<std::string, EsrParam> params;
-  std::vector<std::string> order;
+  Arena arena{256};
+  size_t cap = 0;
+  ParamTable params;
   EsrConv first, body_conv, up1, up2, hr, last;
   std::vector<EsrConv> body;  // [block][rdb][conv]: index (i * 3 + r) * 5 + k
   uint8_t *P = nullptr, *Q = nullptr;
   __half *X[3] = {nullptr, nullptr, nullptr}, *Bc = nullptr, *Cc = nullptr, *t = nullptr, *u1 = nullptr, *u2 = nullptr,
          *h = nullptr;
-  std::vector<GemmLaunch> gemms;  // the static op list between conv_first and conv_last, planned at bind time
-  std::vector<std::string> tags;
-  cudaGraphExec_t graph_exec = nullptr;
+  OpList gemms;  // the static GEMM sequence between conv_first and conv_last, planned at bind time
+  GraphCache graph;
 
-  template <typename T>
-  T* take(size_t n) {
-    used = (used + 255) & ~size_t(255);
-    T* p = dry ? nullptr : reinterpret_cast<T*>(base + used);
-    used += n * sizeof(T);
-    return p;
-  }
-  void reg(const std::string& name, void* dst, int64_t numel, int kind, int N = 0, int C = 0, float scale = 1.f) {
-    EsrParam p;
-    p.dst = dst; p.numel = numel; p.kind = kind; p.N = N; p.C = C; p.scale = scale;
-    if (!params.count(name)) order.push_back(name);
-    params[name] = p;
-  }
   static int64_t cp(int C) { return (C + 63) / 64 * 64; }
   EsrConv conv3(const std::string& name, int N, int C, float bias_scale = 1.f) {
     EsrConv c;
-    c.w = take<__half>(static_cast<size_t>(N) * 9 * cp(C));
-    c.b = take<float>(N);
-    reg(name + ".weight", c.w, static_cast<int64_t>(N) * C * 9, K_CONV3, N, C);
-    reg(name + ".bias", c.b, N, K_BIAS, N, 0, bias_scale);
+    c.w = arena.take<__half>(static_cast<size_t>(N) * 9 * cp(C));
+    c.b = arena.take<float>(N);
+    params.add(name + ".weight", PACKED, c.w, static_cast<int64_t>(N) * C * 9, N, C, 3, 3);
+    params.add(name + ".bias", VEC, c.b, N, N, 0, 1, 1, 0, bias_scale);
     return c;
   }
   EsrConv conv_up(const std::string& name, int N, int C) {
     EsrConv c;
-    c.w = take<__half>(static_cast<size_t>(4) * N * 4 * cp(C));
-    c.b = take<float>(N);
-    reg(name + ".weight", c.w, static_cast<int64_t>(N) * C * 9, K_UP4, N, C);
-    reg(name + ".bias", c.b, N, K_BIAS, N);
+    c.w = arena.take<__half>(static_cast<size_t>(4) * N * 4 * cp(C));
+    c.b = arena.take<float>(N);
+    params.add(name + ".weight", PACKED_UP4, c.w, static_cast<int64_t>(N) * C * 9, N, C);
+    params.add(name + ".bias", VEC, c.b, N);
     return c;
   }
   EsrConv conv_raw(const std::string& name, int N, int C) {
     EsrConv c;
-    c.w = take<__half>(static_cast<size_t>(N) * C * 9);
-    c.b = take<float>(N);
-    reg(name + ".weight", c.w, static_cast<int64_t>(N) * C * 9, K_RAW, N, C);
-    reg(name + ".bias", c.b, N, K_BIAS, N);
+    c.w = arena.take<__half>(static_cast<size_t>(N) * C * 9);
+    c.b = arena.take<float>(N);
+    params.add(name + ".weight", RAW, c.w, static_cast<int64_t>(N) * C * 9);
+    params.add(name + ".bias", VEC, c.b, N);
     return c;
   }
   int64_t pix() const { return static_cast<int64_t>(cfg.frames) * cfg.in_h * cfg.in_w; }
-  void layout() {
+  void layout(void* base) {
     const int nf = cfg.num_feat, gc = cfg.num_grow_ch;
-    used = 0;
-    params.clear();
-    order.clear();
+    arena.reset(base);
+    params.clear(base != nullptr);
     body.assign(static_cast<size_t>(cfg.num_block) * 15, EsrConv{});
     first = conv_raw("conv_first", nf, 3);
     for (int i = 0; i < cfg.num_block; ++i)
@@ -139,9 +106,9 @@ struct EsrEngine {
     const size_t big = ((static_cast<size_t>(pix()) * 16 * nf * 2 + 255) & ~size_t(255));
     const size_t tb = ((static_cast<size_t>(pix()) * nf * 2 + 255) & ~size_t(255));
     const size_t u1b = ((static_cast<size_t>(pix()) * 4 * nf * 2 + 255) & ~size_t(255));
-    P = take<uint8_t>(std::max(5 * catb, big));
-    Q = take<uint8_t>(std::max(tb + u1b, big));
-    if (!dry) {
+    P = arena.take<uint8_t>(std::max(5 * catb, big));
+    Q = arena.take<uint8_t>(std::max(tb + u1b, big));
+    if (base) {
       for (int j = 0; j < 3; ++j) X[j] = reinterpret_cast<__half*>(P + j * catb);
       Bc = reinterpret_cast<__half*>(P + 3 * catb);
       Cc = reinterpret_cast<__half*>(P + 4 * catb);
@@ -163,21 +130,20 @@ struct EsrEngine {
     return d;
   }
   int add(const GemmDesc& d, const std::string& tag) {
-    GemmLaunch L;
-    if (int e = plan_gemm(d, &L)) {
+    auto L = std::make_shared<GemmLaunch>();
+    if (int e = plan_gemm(d, L.get())) {
       set_error(tag + ": " + last_error());
       return e;
     }
-    gemms.push_back(L);
-    tags.push_back(tag);
+    gemms.ops.push_back([L](cudaStream_t st, int) { return launch_gemm(*L, st); });
+    gemms.tags.push_back(tag);
+    gemms.launches += 1;
     return 0;
   }
   int build_ops() {
     gemms.clear();
-    tags.clear();
     const int nf = cfg.num_feat, gc = cfg.num_grow_ch, cat = nf + 4 * gc;
     const int W = cfg.in_w, H = cfg.in_h;
-    gemms.reserve(static_cast<size_t>(cfg.num_block) * 15 + 10);
     int cur = 0;  // X[cur] holds the RRDB input; X[0] = feat stays untouched
     for (int i = 0; i < cfg.num_block; ++i) {
       const int nxt = cur == 1 ? 2 : 1;
@@ -233,12 +199,6 @@ struct EsrEngine {
   }
 };
 
-int run_gemms(EsrEngine* E, cudaStream_t st) {
-  for (const GemmLaunch& L : E->gemms)
-    if (int rc = launch_gemm(L, st)) return rc;
-  return 0;
-}
-
 }  // namespace
 }  // namespace sdw
 
@@ -266,18 +226,13 @@ int sdw_upsampler_create(const sdw_upsampler_config* cfg, sdw_upsampler** out) {
   SDW_REQUIRE(static_cast<int64_t>(cfg->in_h) * cfg->in_w * cfg->frames * 16 < (int64_t(1) << 31), "output too large");
   EsrEngine* E = new EsrEngine();
   E->cfg = *cfg;
-  E->dry = true;
-  E->layout();
-  E->cap = E->used;
+  E->layout(nullptr);
+  E->cap = E->arena.off;
   *out = reinterpret_cast<sdw_upsampler*>(E);
   return 0;
 }
 
-void sdw_upsampler_destroy(sdw_upsampler* e) {
-  EsrEngine* E = reinterpret_cast<EsrEngine*>(e);
-  if (E && E->graph_exec) cudaGraphExecDestroy(E->graph_exec);
-  delete E;
-}
+void sdw_upsampler_destroy(sdw_upsampler* e) { delete reinterpret_cast<EsrEngine*>(e); }
 
 int sdw_upsampler_arena_bytes(const sdw_upsampler* e, uint64_t* bytes) {
   const EsrEngine* E = reinterpret_cast<const EsrEngine*>(e);
@@ -291,70 +246,34 @@ int sdw_upsampler_bind(sdw_upsampler* e, void* arena, uint64_t bytes) {
   SDW_REQUIRE(E && arena, "null");
   SDW_REQUIRE(bytes >= E->cap + 256, "arena too small");
   SDW_REQUIRE((reinterpret_cast<uintptr_t>(arena) & 255) == 0, "arena must be 256-byte aligned");
-  if (E->graph_exec) {
-    cudaGraphExecDestroy(E->graph_exec);
-    E->graph_exec = nullptr;
-  }
-  E->base = static_cast<uint8_t*>(arena);
-  E->dry = false;
-  E->layout();
+  E->graph.reset();
+  E->layout(arena);
   return E->build_ops();
 }
 
 int sdw_upsampler_num_params(const sdw_upsampler* e) {
-  const EsrEngine* E = reinterpret_cast<const EsrEngine*>(e);
-  return E ? static_cast<int>(E->order.size()) : 0;
+  return e ? reinterpret_cast<const EsrEngine*>(e)->params.size() : 0;
 }
 
 int sdw_upsampler_param_info(const sdw_upsampler* e, int index, const char** name, int64_t* numel) {
-  const EsrEngine* E = reinterpret_cast<const EsrEngine*>(e);
-  SDW_REQUIRE(E && index >= 0 && index < static_cast<int>(E->order.size()), "bad index");
-  if (name) *name = E->order[index].c_str();
-  if (numel) *numel = E->params.at(E->order[index]).numel;
-  return 0;
+  SDW_REQUIRE(e, "null");
+  return reinterpret_cast<const EsrEngine*>(e)->params.info(index, name, numel);
 }
 
 int sdw_upsampler_load_param(sdw_upsampler* e, const char* name, const void* src_f16, int64_t numel, void* stream) {
-  EsrEngine* E = reinterpret_cast<EsrEngine*>(e);
-  SDW_REQUIRE(E && name && src_f16 && !E->dry, "null / engine not bound");
-  auto it = E->params.find(name);
-  SDW_REQUIRE(it != E->params.end(), "unknown upsampler parameter");
-  EsrParam& p = it->second;
-  SDW_REQUIRE(numel == p.numel, "upsampler parameter size mismatch");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (p.kind == K_BIAS) {
-    esr_bias_kernel<<<static_cast<unsigned>((numel + 255) / 256), 256, 0, st>>>(static_cast<const __half*>(src_f16),
-                                                                               static_cast<float*>(p.dst),
-                                                                               static_cast<int>(numel), p.scale);
-    SDW_CUDA_OK(cudaGetLastError());
-  } else if (p.kind == K_CONV3) {
-    if (int rc = pack_weight(src_f16, p.N, p.C, 3, 3, 0, p.dst, st)) return rc;
-  } else if (p.kind == K_UP4) {
-    if (int rc = pack_weight_up4(src_f16, p.N, p.C, p.dst, st)) return rc;
-  } else {
-    SDW_CUDA_OK(cudaMemcpyAsync(p.dst, src_f16, static_cast<size_t>(numel) * 2, cudaMemcpyDeviceToDevice, st));
-  }
-  p.loaded = true;
-  return 0;
+  SDW_REQUIRE(e, "null");
+  return reinterpret_cast<EsrEngine*>(e)->params.load(name, src_f16, numel, static_cast<cudaStream_t>(stream));
 }
 
 int sdw_upsampler_missing_params(const sdw_upsampler* e, const char** first_missing) {
-  const EsrEngine* E = reinterpret_cast<const EsrEngine*>(e);
-  if (!E) return -1;
-  int n = 0;
-  for (auto& name : E->order)
-    if (!E->params.at(name).loaded) {
-      if (n == 0 && first_missing) *first_missing = name.c_str();
-      ++n;
-    }
-  return n;
+  return e ? reinterpret_cast<const EsrEngine*>(e)->params.missing(first_missing) : -1;
 }
 
 int sdw_upsampler_run(sdw_upsampler* e, const uint8_t* in_u8, uint8_t* out_u8, float* out_preclamp_f32, int use_graph,
                       void* stream) {
   EsrEngine* E = reinterpret_cast<EsrEngine*>(e);
-  SDW_REQUIRE(E && in_u8 && out_u8 && !E->dry, "null / engine not bound");
-  SDW_REQUIRE(sdw_upsampler_missing_params(e, nullptr) == 0, "upsampler parameters not loaded");
+  SDW_REQUIRE(E && in_u8 && out_u8 && E->params.bound, "null / engine not bound");
+  SDW_REQUIRE(E->params.missing(nullptr) == 0, "upsampler parameters not loaded");
   const sdw_upsampler_config& c = E->cfg;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   SDW_REQUIRE(!use_graph || st != nullptr, "graph capture needs a real stream, not the legacy default stream 0");
@@ -364,22 +283,9 @@ int sdw_upsampler_run(sdw_upsampler* e, const uint8_t* in_u8, uint8_t* out_u8, f
                              c.num_feat + 4 * c.num_grow_ch, st))
     return rc;
   if (use_graph) {
-    if (!E->graph_exec) {
-      cudaGraph_t graph = nullptr;
-      SDW_CUDA_OK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      int rc = run_gemms(E, st);
-      cudaError_t ce = cudaStreamEndCapture(st, &graph);
-      if (rc) {
-        if (graph) cudaGraphDestroy(graph);
-        return rc;
-      }
-      SDW_CUDA_OK(ce);
-      SDW_CUDA_OK(cudaGraphInstantiate(&E->graph_exec, graph, 0));
-      cudaGraphDestroy(graph);
-    }
-    SDW_CUDA_OK(cudaGraphLaunch(E->graph_exec, st));
+    if (int rc = E->graph.launch(0, st, [E](cudaStream_t s) { return E->gemms.run(s, 0); })) return rc;
   } else {
-    if (int rc = run_gemms(E, st)) return rc;
+    if (int rc = E->gemms.run(st, 0)) return rc;
   }
   return conv_out_small(E->h, c.num_feat, c.frames, 4 * c.in_h, 4 * c.in_w, c.num_feat, E->last.w, E->last.b, 3,
                         out_preclamp_f32, out_u8, st, 1);
@@ -389,48 +295,27 @@ int sdw_upsampler_run(sdw_upsampler* e, const uint8_t* in_u8, uint8_t* out_u8, f
 // microseconds<TAB>tag" lines.  The edge convs read / write dead arena regions here (their values do not matter).
 int sdw_upsampler_debug_profile(sdw_upsampler* e, const char* path, void* stream) {
   EsrEngine* E = reinterpret_cast<EsrEngine*>(e);
-  SDW_REQUIRE(E && path && !E->dry, "engine not bound");
-  SDW_REQUIRE(sdw_upsampler_missing_params(e, nullptr) == 0, "upsampler parameters not loaded");
+  SDW_REQUIRE(E && path && E->params.bound, "engine not bound");
+  SDW_REQUIRE(E->params.missing(nullptr) == 0, "upsampler parameters not loaded");
   const sdw_upsampler_config& c = E->cfg;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  std::vector<std::function<int()>> ops;
-  std::vector<std::string> tags;
   const uint8_t* in_scratch = E->Q;  // dead while conv_first runs
   uint8_t* out_scratch = E->P;       // dead while conv_last runs
-  ops.push_back([=] {
+  OpList ops;
+  ops.ops.push_back([=](cudaStream_t st, int) {
     return conv_first_u8(in_scratch, c.frames, c.in_h, c.in_w, E->first.w, E->first.b, c.num_feat, E->X[0],
                          c.num_feat + 4 * c.num_grow_ch, st);
   });
-  tags.push_back("conv_first u8 3->64 (CUDA cores)");
-  for (size_t i = 0; i < E->gemms.size(); ++i) {
-    ops.push_back([=] { return launch_gemm(E->gemms[i], st); });
-    tags.push_back(E->tags[i]);
-  }
-  ops.push_back([=] {
+  ops.tags.push_back("conv_first u8 3->64 (CUDA cores)");
+  ops.ops.insert(ops.ops.end(), E->gemms.ops.begin(), E->gemms.ops.end());
+  ops.tags.insert(ops.tags.end(), E->gemms.tags.begin(), E->gemms.tags.end());
+  ops.ops.push_back([=](cudaStream_t st, int) {
     return conv_out_small(E->h, c.num_feat, c.frames, 4 * c.in_h, 4 * c.in_w, c.num_feat, E->last.w, E->last.b, 3,
                           nullptr, out_scratch, st, 1);
   });
-  tags.push_back("conv_last 64->3 + uint8 (CUDA cores)");
-  for (auto& op : ops)
-    if (int rc = op()) return rc;
+  ops.tags.push_back("conv_last 64->3 + uint8 (CUDA cores)");
   FILE* f = std::fopen(path, "w");
   SDW_REQUIRE(f, "cannot open the profile file");
-  const size_t n = ops.size();
-  std::vector<cudaEvent_t> ev(n + 1);
-  for (auto& x : ev) cudaEventCreate(&x);
-  int rc = 0;
-  cudaEventRecord(ev[0], st);
-  for (size_t i = 0; i < n && !rc; ++i) {
-    rc = ops[i]();
-    cudaEventRecord(ev[i + 1], st);
-  }
-  cudaStreamSynchronize(st);
-  for (size_t i = 0; i < n && !rc; ++i) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-    std::fprintf(f, "upsampler\t%zu\t%.2f\t%s\n", i, ms * 1e3f, tags[i].c_str());
-  }
-  for (auto& x : ev) cudaEventDestroy(x);
+  int rc = profile_ops(f, "upsampler", ops, static_cast<cudaStream_t>(stream), 0);
   std::fclose(f);
   if (rc) return rc;
   SDW_CUDA_OK(cudaGetLastError());

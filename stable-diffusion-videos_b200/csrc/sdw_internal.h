@@ -6,7 +6,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cstdio>
+#include <functional>
 #include <string>
+#include <unordered_map>
+#include <vector>
 
 namespace sdw {
 
@@ -257,6 +261,88 @@ int vae_in(const float* x, float inv_scale, const __half* w, const float* bias, 
 int linear_f32(const float* in, int64_t ldi, const __half* w, const float* bias, int M, int N, int K, int silu_in,
                int silu_out, float* out, int64_t ldo, cudaStream_t stream);
 int timestep_embed(const float* t, int n, int dim, int round_f16, float* out, cudaStream_t stream);
-int half_to_float(const __half* in, float* out, int64_t n, int geglu_N, cudaStream_t stream);
+// out[i] = fp32(in[i]) * scale; geglu_N > 0 permutes the rows as pack_weight does for a GEGLU projection of N rows
+int half_to_float(const __half* in, float* out, int64_t n, int geglu_N, float scale, cudaStream_t stream);
+
+// ---------------------------------------------------------------------------
+// host scaffolding of the engines (sdw_model.cu): arena layout, parameter table, op lists, graph replay, profiling
+// ---------------------------------------------------------------------------
+// Bump allocator over a caller-owned arena.  With no base (the dry run) it only measures: take() returns null.
+struct Arena {
+  explicit Arena(size_t align) : align(align) {}
+  size_t align;
+  uint8_t* base = nullptr;
+  size_t off = 0, peak = 0;
+  void reset(void* b) {
+    base = static_cast<uint8_t*>(b);
+    off = peak = 0;
+  }
+  void* take(size_t bytes);
+  template <typename T>
+  T* take(size_t n) {
+    return static_cast<T*>(take(n * sizeof(T)));
+  }
+};
+
+// How a checkpoint tensor (fp16, its own layout) reaches its arena slot.
+enum ParamKind : int {
+  PACKED,      // conv / linear weight -> pack_weight (kh x kw taps, geglu row interleave)
+  PACKED_UP4,  // nearest-up2 + 3x3 conv weight -> pack_weight_up4
+  RAW,         // fp16 copy
+  VEC,         // fp32 vector x scale; geglu: rows permuted like the packed GEGLU weight of N rows
+};
+struct Param {
+  std::string name;
+  ParamKind kind;
+  void* dst;
+  int64_t numel;
+  int N, C, kh, kw, geglu;
+  float scale;
+  bool loaded;
+};
+// name -> slot, in registration order; re-registering a name replaces its slot and keeps its position
+struct ParamTable {
+  bool bound = false;  // slots point into a bound arena (else the dry run's nulls)
+  std::vector<Param> slots;
+  std::unordered_map<std::string, int> index;
+  void clear(bool bound_arena);
+  void add(const std::string& name, ParamKind kind, void* dst, int64_t numel, int N = 0, int C = 0, int kh = 1,
+           int kw = 1, int geglu = 0, float scale = 1.f);
+  int size() const { return static_cast<int>(slots.size()); }
+  int info(int i, const char** name, int64_t* numel) const;
+  Param* find(const std::string& name);
+  int missing(const char** first) const;
+  // validates name, binding and numel before anything is launched
+  int load(const char* name, const void* src_f16, int64_t numel, cudaStream_t stream);
+};
+
+// a static launch sequence: op(stream, step) closures, a tag per op (profiles), and the kernel launches it makes
+using OpFn = std::function<int(cudaStream_t, int /*step*/)>;
+struct OpList {
+  std::vector<OpFn> ops;
+  std::vector<std::string> tags;
+  int launches = 0;
+  void clear() {
+    ops.clear();
+    tags.clear();
+    launches = 0;
+  }
+  int run(cudaStream_t st, int step) const;
+};
+
+// one instantiated CUDA graph of `body`, re-captured when the key changes
+struct GraphCache {
+  cudaGraphExec_t exec = nullptr;
+  int key = -1;
+  GraphCache() = default;
+  GraphCache(const GraphCache&) = delete;
+  GraphCache& operator=(const GraphCache&) = delete;
+  ~GraphCache() { reset(); }
+  void reset();
+  int launch(int k, cudaStream_t st, const std::function<int(cudaStream_t)>& body);
+};
+
+// tooling: one untimed pass of `ops`, then CUDA events around every op; writes "section<TAB>index<TAB>us<TAB>tag" lines
+int profile_ops(FILE* f, const char* section, const OpList& ops, cudaStream_t st, int step);
 
 }  // namespace sdw

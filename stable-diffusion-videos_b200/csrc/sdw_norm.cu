@@ -904,9 +904,8 @@ int timestep_embed(const float* t, int n, int dim, int round_f16, float* out, cu
   return 0;
 }
 
-// fp16 -> fp32 vector conversion (biases, norm affine parameters)
-__global__ void h2f_kernel(const __half* __restrict__ in, float* __restrict__ out, int64_t n, const int* perm_geglu,
-                           int N) {
+// fp16 -> fp32 vector conversion (biases, norm affine parameters), times `scale` (1 is an exact identity)
+__global__ void h2f_kernel(const __half* __restrict__ in, float* __restrict__ out, int64_t n, int N, float scale) {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n) return;
   int64_t src = i;
@@ -915,11 +914,11 @@ __global__ void h2f_kernel(const __half* __restrict__ in, float* __restrict__ ou
     const int blk = r >> 6, within = r & 63;
     src = within < 32 ? blk * 32 + within : N / 2 + blk * 32 + (within - 32);
   }
-  out[i] = __half2float(in[src]);
+  out[i] = __half2float(in[src]) * scale;
 }
 
-int half_to_float(const __half* in, float* out, int64_t n, int geglu_N, cudaStream_t stream) {
-  h2f_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(in, out, n, nullptr, geglu_N);
+int half_to_float(const __half* in, float* out, int64_t n, int geglu_N, float scale, cudaStream_t stream) {
+  h2f_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(in, out, n, geglu_N, scale);
   SDW_CUDA_OK(cudaGetLastError());
   return 0;
 }

@@ -60,43 +60,19 @@ class Engine:
         c.tiled = int(bool(tiled))  # circular convolution padding (reference from_pretrained(tiled=True), P:841-858)
         self.cfg = c
         self.vae_scale = c.vae_scale
-        lib = N.lib()
-        self._h = C.c_void_p()
-        N.check(lib.sdw_engine_create(C.byref(c), C.byref(self._h)))
-        nbytes = C.c_uint64()
-        N.check(lib.sdw_engine_arena_bytes(self._h, C.byref(nbytes)))
-        self.arena_bytes = int(nbytes.value)
-        with torch.cuda.device(self.device):
-            self.arena = torch.zeros(self.arena_bytes + 1024, dtype=torch.uint8, device=self.device)
-            base = (self.arena.data_ptr() + 1023) // 1024 * 1024
-            N.check(lib.sdw_engine_bind(self._h, C.c_void_p(base), C.c_uint64(self.arena_bytes)))
+        self._model = N.NativeModel("engine", c, 1024, self.device, "UNet / VAE")
+        self._h = self._model.h
         self.n_steps = 0
         self._plan_key = None
         # graph capture is illegal on the legacy default stream: the engine runs on its own stream, fenced both ways
         self._stream = torch.cuda.Stream(device=self.device)
 
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                N.lib().sdw_engine_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
-
     # ------------------------------------------------------------------------------------------
     def param_names(self):
-        lib = N.lib()
-        out = {}
-        name, numel = C.c_char_p(), C.c_int64()
-        for i in range(lib.sdw_engine_num_params(self._h)):
-            N.check(lib.sdw_engine_param_info(self._h, i, C.byref(name), C.byref(numel)))
-            out[name.value.decode()] = int(numel.value)
-        return out
+        return self._model.param_names()
 
     def load_state_dict(self, unet_sd, vae_sd, strict=True):
         """unet_sd: diffusers UNet keys; vae_sd: AutoencoderKL keys (post_quant_conv.*, decoder.*; encoder ignored)."""
-        lib = N.lib()
-        expected = self.param_names()
         shapes = dict(unet_param_shapes(self.unet_cfg))
         shapes.update({"vae." + k: v for k, v in vae_param_shapes(self.vae_cfg).items()})
         items = dict(unet_sd)
@@ -106,27 +82,15 @@ class Engine:
             parts = k.split(".")
             parts = [VAE_KEY_ALIASES.get(p, p) for p in parts]
             items["vae." + ".".join(parts)] = v
-        keep = []
-        with torch.cuda.device(self.device):
-            for name, t in items.items():
-                if name not in expected:
-                    if strict:
-                        raise N.SdwError(f"unexpected parameter {name}")
-                    continue
-                want, got = tuple(shapes[name]), tuple(t.shape)
-                # the only accepted alias: a 1x1 conv stored as a Linear weight or the reverse, (c_out, c_in) <->
-                # (c_out, c_in, 1, 1) (old VAE attention checkpoints, use_linear_projection models)
-                if got != want and got + (1, 1) != want and got != want + (1, 1):
-                    raise N.SdwError(f"shape mismatch for {name}: {got} vs {want}")
-                th = t.detach().to(device=self.device, dtype=torch.float16).contiguous()
-                keep.append(th)
-                N.check(lib.sdw_engine_load_param(self._h, name.encode(), N.ptr(th), C.c_int64(th.numel()),
-                                                  N.stream_ptr()))
-            torch.cuda.current_stream().synchronize()
-        first = C.c_char_p()
-        missing = lib.sdw_engine_missing_params(self._h, C.byref(first))
-        if missing:
-            raise N.SdwError(f"{missing} parameters not loaded (first: {first.value.decode()})")
+        for name, t in items.items():
+            if name not in shapes:
+                continue  # the engine's table is the same key set: load() rejects or skips it
+            want, got = tuple(shapes[name]), tuple(t.shape)
+            # the only accepted alias: a 1x1 conv stored as a Linear weight or the reverse, (c_out, c_in) <->
+            # (c_out, c_in, 1, 1) (old VAE attention checkpoints, use_linear_projection models)
+            if got != want and got + (1, 1) != want and got != want + (1, 1):
+                raise N.SdwError(f"shape mismatch for {name}: {got} vs {want}")
+        self._model.load(items, strict)
 
     def set_scheduler(self, scheduler, num_inference_steps, guidance_scale):
         scheduler.set_timesteps(num_inference_steps)

@@ -66,38 +66,11 @@ class UpsamplerEngine:
     def __init__(self, state_dict, num_block, h, w, frames, device):
         self.device = torch.device(device)
         self.h, self.w, self.frames = int(h), int(w), int(frames)
-        lib = N.lib()
-        lib.sdw_upsampler_destroy.restype = None
         self.cfg = UpsamplerConfig(64, int(num_block), 32, self.h, self.w, self.frames)
-        self._h = C.c_void_p()
-        N.check(lib.sdw_upsampler_create(C.byref(self.cfg), C.byref(self._h)))
+        self._model = N.NativeModel("upsampler", self.cfg, 256, self.device, "upsampler")
+        self._h = self._model.h
         self.stream = torch.cuda.Stream(device=self.device)
-        nbytes = C.c_uint64()
-        N.check(lib.sdw_upsampler_arena_bytes(self._h, C.byref(nbytes)))
-        self.arena_bytes = int(nbytes.value)
-        with torch.cuda.device(self.device):
-            self.arena = torch.empty(self.arena_bytes + 256, dtype=torch.uint8, device=self.device)
-            base = (self.arena.data_ptr() + 255) // 256 * 256
-            N.check(lib.sdw_upsampler_bind(self._h, C.c_void_p(base), C.c_uint64(self.arena_bytes)))
-            keep = []
-            for name, t in state_dict.items():
-                th = t.to(device=self.device, dtype=torch.float16).contiguous()
-                keep.append(th)
-                N.check(lib.sdw_upsampler_load_param(self._h, name.encode(), N.ptr(th), C.c_int64(th.numel()),
-                                                     N.stream_ptr()))
-            torch.cuda.current_stream().synchronize()
-        first = C.c_char_p()
-        missing = lib.sdw_upsampler_missing_params(self._h, C.byref(first))
-        if missing:
-            raise N.SdwError(f"{missing} upsampler parameters not loaded (first: {first.value.decode()})")
-
-    def __del__(self):
-        try:
-            if getattr(self, "_h", None):
-                N.lib().sdw_upsampler_destroy(self._h)
-                self._h = None
-        except Exception:
-            pass
+        self._model.load(state_dict)
 
     def run(self, u8_in, u8_out, preclamp=None, use_graph=True):
         """u8_in [frames, H, W, 3] -> u8_out [frames, 4H, 4W, 3] (and the fp32 pre-clamp output), ordered after the
