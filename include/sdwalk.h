@@ -12,7 +12,8 @@
  *   - all buffers are caller-owned DEVICE pointers (torch tensors' data_ptr()), sizes explicit.
  *   - `stream` is a cudaStream_t passed as void* (torch.cuda.current_stream().cuda_stream).
  *   - no entry point synchronises the device or allocates device memory, except
- *     sdw_engine_create (records sizes only) — the arena is supplied by the caller.
+ *     sdw_engine_create (records sizes only) and the first safety-checker call for a frame size (its resize buffer,
+ *     see sdw_safety_check) — the arena is supplied by the caller.
  *   - one engine per (process, device); an engine is not thread-safe (mirrors the reference:
  *     mutable scheduler state, stable_diffusion_pipeline.py:394).
  */
@@ -333,6 +334,59 @@ int sdw_conv_first_u8(const uint8_t* x, int B, int H, int W, const void* w, cons
                       void* stream);
 int sdw_conv_last_u8(const void* x, int64_t ldx, int B, int H, int W, int C, const void* w, const float* bias,
                      float* out_f32, uint8_t* out_u8, void* stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Stable Diffusion safety checker: replaces `self.feature_extractor(...)` + `self.safety_checker(...)` of __call__
+ * (stable_diffusion_pipeline.py:440-447; diffusers' StableDiffusionSafetyChecker on a CLIPVisionModel).  Parameter names
+ * are its state-dict keys ("vision_model.vision_model.embeddings.patch_embedding.weight", ...,
+ * "visual_projection.weight", "concept_embeds", "special_care_embeds", "concept_embeds_weights",
+ * "special_care_embeds_weights"), handed over as fp16.  Life cycle as the CLIP text tower.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct sdw_safety sdw_safety;
+typedef struct sdw_safety_config {
+  int32_t hidden, layers, heads, intermediate; /* hidden = 64 heads */
+  int32_t image_size, patch;                   /* image_size 224 (the crop); patch divides it */
+  int32_t proj_dim, n_concepts, n_special;     /* n_concepts + n_special <= 64 */
+  float eps;                                   /* LayerNorm epsilon */
+  int32_t max_batch;                           /* frames per tower pass; larger calls run in chunks */
+  int32_t act;                                 /* 0: quick-GELU (ViT-L/14), 1: erf GELU */
+  float mean[3], std[3];                       /* the feature extractor's image_mean / image_std */
+} sdw_safety_config;
+int sdw_safety_create(const sdw_safety_config* cfg, sdw_safety** out);
+void sdw_safety_destroy(sdw_safety* e);
+int sdw_safety_arena_bytes(const sdw_safety* e, uint64_t* bytes);
+int sdw_safety_bind(sdw_safety* e, void* arena, uint64_t bytes);
+/* parameter table as the sampler engine's */
+int sdw_safety_num_params(const sdw_safety* e);
+int sdw_safety_param_info(const sdw_safety* e, int index, const char** name, int64_t* numel);
+int sdw_safety_load_param(sdw_safety* e, const char* name, const void* data_f16, int64_t numel, void* stream);
+int sdw_safety_missing_params(const sdw_safety* e, const char** first_missing);
+/* frames_u8: device uint8 RGB [B][H][W][3]; flags: device int32 [B] (1 = an NSFW concept was detected);
+ * cos_f32 (optional): device fp32 [B][n_special + n_concepts] cosine similarities, special-care concepts first;
+ * blackout = 1 zeroes the flagged frames in place.  Any B (chunks of max_batch).  The first call for a frame size
+ * (H, W) is synchronous: it allocates the resize buffer (outside the arena; cudaFree of the previous size's) and uploads
+ * Pillow's coefficient tables; later calls at that size only enqueue work.  The tower of each chunk size replays as a
+ * CUDA graph, captured on its first call (`stream` must be a real stream). */
+int sdw_safety_check(sdw_safety* e, void* frames_u8, int B, int H, int W, int32_t* flags, float* cos_f32, int blackout,
+                     void* stream);
+/* the checker's stages on their own (tests / tooling):
+ *   safety_preprocess : B <= max_batch frames -> pixels_f16 (optional) [B][224][224][3] normalised pixels, crop_u8
+ *                       (optional) [B][224][224][3] the Pillow-resized, centre-cropped uint8 image, patch_rows_f16
+ *                       (optional) [B * patches][ceil64(3 patch^2)] the patch GEMM's A operand, written by the
+ *                       normalisation kernel itself (pad columns included)
+ *   safety_embed      : image_embeds fp32 [B][proj_dim] (any B); use_graph = 0 runs the ops eagerly
+ *   safety_scores     : the score kernel on given fp32 tables: special [ns][D], special_w [ns], concepts [nc][D],
+ *                       concept_w [nc]; flags [B], cos_f32 / scores_f64 [B][ns + nc] optional, and frames_u8
+ *                       (optional, frame_bytes each) zeroed where flagged */
+int sdw_safety_preprocess(sdw_safety* e, const uint8_t* frames_u8, int B, int H, int W, void* pixels_f16, uint8_t* crop_u8,
+                          void* patch_rows_f16, void* stream);
+int sdw_safety_embed(sdw_safety* e, const uint8_t* frames_u8, int B, int H, int W, float* embeds_f32, int use_graph,
+                     void* stream);
+int sdw_safety_scores(const float* embeds_f32, int B, int D, const float* special, const float* special_w, int ns,
+                      const float* concepts, const float* concept_w, int nc, int32_t* flags, float* cos_f32,
+                      double* scores_f64, uint8_t* frames_u8, int64_t frame_bytes, void* stream);
+/* tooling: CUDA-event time of every op of one check of B <= max_batch frames, written as TSV to `path` */
+int sdw_safety_debug_profile(sdw_safety* e, const uint8_t* frames_u8, int B, int H, int W, const char* path, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Frame-sharded walk over the GPUs of one box (one process per GPU): the three exchanges of the path, as thin NCCL

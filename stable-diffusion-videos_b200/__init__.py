@@ -18,6 +18,7 @@ _LAZY = {
     "UNetConfig": ("configs", "UNetConfig"),
     "VAEConfig": ("configs", "VAEConfig"),
     "RealESRGANModel": ("upsampling", "RealESRGANModel"),
+    "NativeSafetyChecker": ("safety", "NativeSafetyChecker"),
 }
 
 

@@ -76,7 +76,7 @@ def require_cuda(*tensors):
 
 
 class NativeModel:
-    """One native engine behind the `sdw_<prefix>_*` functions (engine, clip, upsampler): created from its config
+    """One native engine behind the `sdw_<prefix>_*` functions (engine, clip, upsampler, safety): created from its config
     struct, bound to a zero-filled arena on `device` aligned to `align` bytes, destroyed with this object.  `h` is the
     handle the engine's own entry points take; `what` names the model in error messages."""
 
@@ -217,3 +217,28 @@ def clip_act(x, n, gelu_erf):
     """in place over the first n fp16 values of x: quick-GELU (gelu_erf = 0) or erf GELU (1)."""
     require_cuda(x)
     check(lib().sdw_clip_act(ptr(x), C.c_int64(n), C.c_int(int(gelu_erf)), stream_ptr()))
+
+
+def safety_patch_rows(h, frames_u8, rows):
+    """the safety checker's patch GEMM operand for frames_u8 [B, H, W, 3] (B <= max_batch), written into `rows`
+    (fp16 [B * patches, ceil64(3 patch^2)])"""
+    require_cuda(frames_u8, rows)
+    B, H, W = frames_u8.shape[:3]
+    check(lib().sdw_safety_preprocess(h, ptr(frames_u8), B, H, W, None, None, ptr(rows), stream_ptr()))
+
+
+def safety_scores(embeds, special, special_w, concepts, concept_w, frames_u8=None):
+    """the safety checker's score kernel on fp32 tables: returns (flags int32 [B], cos fp32 [B, ns + nc],
+    scores fp64 [B, ns + nc]); flagged frames of `frames_u8` (uint8 [B, ...]) are zeroed in place"""
+    t = [x.float().contiguous() for x in (embeds, special, special_w, concepts, concept_w)]
+    require_cuda(*t, frames_u8)
+    B, D = t[0].shape
+    ns, nc = t[1].shape[0], t[3].shape[0]
+    flags = torch.empty(B, dtype=torch.int32, device=t[0].device)
+    cos = torch.empty((B, ns + nc), dtype=torch.float32, device=t[0].device)
+    sc = torch.empty((B, ns + nc), dtype=torch.float64, device=t[0].device)
+    fb = frames_u8[0].numel() if frames_u8 is not None else 0
+    check(lib().sdw_safety_scores(ptr(t[0]), C.c_int(B), C.c_int(D), ptr(t[1]), ptr(t[2]), C.c_int(ns), ptr(t[3]),
+                                  ptr(t[4]), C.c_int(nc), ptr(flags), ptr(cos), ptr(sc), ptr(frames_u8), C.c_int64(fb),
+                                  stream_ptr()))
+    return flags, cos, sc

@@ -168,10 +168,14 @@ class StableDiffusionWalkPipeline:
                 "Make sure to define a feature extractor when loading {self.__class__} if you want to use the safety"
                 " checker. If you do not want to use the safety checker, you can pass `'safety_checker=None'` instead.")
         if safety_checker is not None:
-            raise NotImplementedError("the native hot path has no safety checker (None in every reference test/example)")
+            from .safety import NativeSafetyChecker
+
+            if not isinstance(safety_checker, NativeSafetyChecker):
+                raise TypeError(f"safety_checker must be a NativeSafetyChecker (the native checker), got "
+                                f"{type(safety_checker).__name__}")
         self.vae, self.text_encoder, self.tokenizer, self.unet = vae, text_encoder, tokenizer, unet
         self.scheduler = scheduler
-        self.safety_checker, self.feature_extractor = None, feature_extractor
+        self.safety_checker, self.feature_extractor = safety_checker, feature_extractor
         self.vae_scale_factor = 2 ** (len(self.vae.config.block_out_channels) - 1)  # P:158
         self.device = torch.device("cpu")
         self.tiled = False
@@ -196,12 +200,20 @@ class StableDiffusionWalkPipeline:
 
     @classmethod
     def from_pretrained(cls, path, *args, tiled=False, torch_dtype=None, safety_checker=None, **kwargs):
-        """Load a LOCAL diffusers-layout checkpoint directory (unet/, vae/, text_encoder/, tokenizer/, scheduler/)."""
+        """Load a LOCAL diffusers-layout checkpoint directory (unet/, vae/, text_encoder/, tokenizer/, scheduler/).
+
+        `safety_checker=True` also loads the checkpoint's safety_checker/ and feature_extractor/ (FileNotFoundError if
+        they are absent); a NativeSafetyChecker is used as given.  The default, None, loads no checker (diffusers loads
+        one by default)."""
         from safetensors.torch import load_file
 
         root = Path(path)
         if not root.is_dir():
             raise FileNotFoundError(f"{path}: from_pretrained needs a local checkpoint directory (no network here)")
+        if safety_checker is True:
+            for sub in ("safety_checker/config.json", "feature_extractor/preprocessor_config.json"):
+                if not (root / sub).is_file():
+                    raise FileNotFoundError(f"safety_checker=True: {root / sub} does not exist")
 
         def _cfg(sub):
             return json.loads((root / sub / "config.json").read_text())
@@ -259,7 +271,16 @@ class StableDiffusionWalkPipeline:
         text_encoder = NativeCLIPTextEncoder.from_hf_model(hf_text)
         del hf_text
         tokenizer = CLIPTokenizer.from_pretrained(str(root / "tokenizer"))
-        pipe = cls(NativeVAE(vcfg, _sd("vae")), text_encoder, tokenizer, NativeUNet(ucfg, _sd("unet")), sch)
+        checker, fe = None, None
+        if safety_checker is True:
+            from .safety import NativeSafetyChecker
+
+            checker = NativeSafetyChecker.from_pretrained(root)
+            fe = json.loads((root / "feature_extractor" / "preprocessor_config.json").read_text())
+        elif safety_checker not in (None, False):
+            checker, fe = safety_checker, kwargs.get("feature_extractor")
+        pipe = cls(NativeVAE(vcfg, _sd("vae")), text_encoder, tokenizer, NativeUNet(ucfg, _sd("unet")), sch,
+                   safety_checker=checker, feature_extractor=fe)
         pipe.tiled = tiled
         return pipe
 
@@ -274,6 +295,10 @@ class StableDiffusionWalkPipeline:
         self._uncond_cache = {}  # embeddings live on the previous device / came from the previous encoder
         if hasattr(self.text_encoder, "to"):
             self.text_encoder = self.text_encoder.to(device)
+        if self.safety_checker is not None and self.safety_checker.device != device:
+            raise _native.SdwError(f"the safety checker lives on {self.safety_checker.device}, where it was built; "
+                                   f"build it on {device} (NativeSafetyChecker(..., device=...)) to run the pipeline "
+                                   "there")
         return self
 
     def enable_attention_slicing(self, slice_size="auto"):  # P:161-180 — memory knob, moot here
@@ -391,6 +416,10 @@ class StableDiffusionWalkPipeline:
         frames_u8, raw = self._sample_device(latents, text_embeddings, uncond, height, width, num_inference_steps,
                                              guidance_scale, want_raw=want_float, callback=callback,
                                              callback_steps=callback_steps)
+        has_nsfw = None
+        if self.safety_checker is not None:  # P:440-447: flagged images become black
+            flags = self.safety_checker.check_frames(frames_u8, blackout=True)
+            has_nsfw = [bool(f) for f in flags.cpu()]
         if output_type == "pil":
             from PIL import Image
 
@@ -398,9 +427,11 @@ class StableDiffusionWalkPipeline:
             image = [Image.fromarray(a) for a in arr]
         else:
             image = (raw / 2 + 0.5).clamp(0, 1).cpu().numpy()  # float32 NHWC in [0,1] (P:435-438)
+            if has_nsfw is not None:
+                image[np.asarray(has_nsfw, dtype=bool)] = 0
         if not return_dict:
-            return (image, None)
-        return StableDiffusionPipelineOutput(images=image, nsfw_content_detected=None)
+            return (image, has_nsfw)
+        return StableDiffusionPipelineOutput(images=image, nsfw_content_detected=has_nsfw)
 
     def _sample_device(self, latents, text_embeddings, uncond, height, width, num_inference_steps, guidance_scale,
                        want_raw=False, callback=None, callback_steps=1):
@@ -489,6 +520,8 @@ class StableDiffusionWalkPipeline:
                 noise_batch = torch.cat([noise_batch, noise_batch[-1:].expand(pad, -1, -1, -1)])
             frames_u8, _ = self._sample_device(noise_batch, embeds_batch, uncond, height, width, num_inference_steps,
                                                guidance_scale)
+            if self.safety_checker is not None:  # flagged frames are saved black (and upsampled black, P:546-552)
+                self.safety_checker.check_frames(frames_u8[:nb], blackout=True)
             if upsample:  # each rank upsamples its own block before the gather
                 frames_u8 = self.upsampler.upsample_frames(frames_u8[:nb])
             if world > 1:
