@@ -164,6 +164,12 @@ int sdw_engine_debug_unet(sdw_engine* e, const float* x_nchw, int step, const vo
 int sdw_engine_debug_vae(sdw_engine* e, const float* latents_nchw, uint8_t* out_u8, float* out_f32_nhwc, void* stream);
 /* tooling: CUDA-event time of every op of one UNet forward and of the VAE decode, written as TSV to `path` */
 int sdw_engine_debug_profile(sdw_engine* e, const char* path, void* stream);
+/* tooling: the launch plan of the UNet and VAE op lists, launching nothing (works in plan-only mode on a fake arena).
+ * One TSV line per kernel-level record: "section<TAB>op index<TAB>kind<TAB>key=value..." (an op that runs several
+ * kernels, such as the tiled edge convs, writes one line per kernel under the same index).  gemm lines carry every
+ * sdw_gemm_desc field that shapes the launch plus the plan (ver bn nsub ew tr et stages) and whether the residual
+ * (res_alias) or the input (in_alias) is the output buffer; attention lines carry the descriptor and the plan. */
+int sdw_engine_debug_ops(const sdw_engine* e, const char* path);
 
 /* ------------------------------------------------------------------------------------------
  * Low-level tensor-core op (tests / tooling): one implicit GEMM on the wgmma kernel.

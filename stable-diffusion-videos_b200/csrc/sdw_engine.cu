@@ -15,6 +15,7 @@
 #include "sdw_internal.h"
 
 #include <cmath>
+#include <cstdarg>
 #include <cstdlib>
 #include <cstring>
 #include <functional>
@@ -27,6 +28,37 @@ int unet_ctx_assemble(const __half* cond, const __half* uncond, int F, int dup, 
                       cudaStream_t stream);
 
 namespace {
+
+// printf into a std::string (op records of sdw_engine_debug_ops)
+std::string strf(const char* fmt, ...) {
+  char buf[1024];
+  va_list ap;
+  va_start(ap, fmt);
+  std::vsnprintf(buf, sizeof buf, fmt, ap);
+  va_end(ap);
+  return buf;
+}
+using ll = long long;
+
+std::string gemm_record(const GemmDesc& d, const GemmLaunch& L, bool rowvec) {
+  return strf("gemm\tC=%d\tW=%d\tH=%d\tB=%d\tsW=%lld\tsH=%lld\tsB=%lld\tconv=%d\tup_px=%d\tup_py=%d\tN=%d\tldb=%lld\tKb=%lld\t"
+              "b_batched=%d\tsBh=%lld\tsBb=%lld\tldc=%lld\to_sW=%lld\to_sH=%lld\to_sB=%lld\tldr=%lld\trowvec_ld=%d\t"
+              "bias=%d\trowvec=%d\tresid=%d\tmode=%d\tact=%d\talpha=%.9g\tvt_col0=%d\tvt_d=%d\tvt_heads=%d\tvt_ntok=%d\t"
+              "vt_ld=%lld\tver=%d\tbn=%d\tnsub=%d\tew=%d\ttr=%d\tet=%d\tstages=%d\tres_alias=%d\tin_alias=%d",
+              d.C, d.W, d.H, d.B, ll(d.sW), ll(d.sH), ll(d.sB), d.conv, d.up_px, d.up_py, d.N, ll(d.ldb), ll(d.Kb),
+              d.b_batched, ll(d.sBh), ll(d.sBb), ll(d.ldc), ll(d.o_sW), ll(d.o_sH), ll(d.o_sB), ll(d.ldr),
+              rowvec ? 0 : d.rowvec_ld, d.bias != nullptr, rowvec || d.rowvec, d.resid != nullptr, d.mode, d.act,
+              static_cast<double>(d.alpha), d.vt_col0, d.vt_d, d.vt_heads, d.vt_ntok, ll(d.vt_ld), L.ver, L.bn, L.nsub,
+              L.ew, L.tr, L.p.epi_tma, L.p.nstages, d.resid != nullptr && d.resid == d.out,
+              d.A == static_cast<const __half*>(d.out));
+}
+std::string wrap_pad_record(int64_t ld_bytes, int B, int H, int W, int pix_bytes, int pad) {
+  return strf("wrap_pad\tld_bytes=%lld\tB=%d\tH=%d\tW=%d\tpix_bytes=%d\tpad=%d", ll(ld_bytes), B, H, W, pix_bytes, pad);
+}
+std::string crop_record(int B, int H, int W, int pix_bytes, int crop, bool resid, int64_t ldr, int64_t ldo_bytes) {
+  return strf("crop\tB=%d\tH=%d\tW=%d\tpix_bytes=%d\tcrop=%d\tresid=%d\tldr=%lld\tldo_bytes=%lld", B, H, W, pix_bytes, crop,
+              int(resid), ll(ldr), ll(ldo_bytes));
+}
 
 struct T {  // NHWC fp16 view
   __half* p = nullptr;
@@ -149,12 +181,15 @@ struct Engine {
   // ---- op emission ---------------------------------------------------------
   OpList* cur = nullptr;
   std::string tag_next;  // names the op about to be emitted (tooling: sdw_engine_debug_profile)
+  std::string rec_next;  // its arguments, one "kind<TAB>key=value..." line per kernel (tooling: sdw_engine_debug_ops)
   void emit(OpFn f, int launches = 1) {
     if (!dry) {
       cur->ops.push_back(std::move(f));
       cur->tags.push_back(tag_next.empty() ? std::string("op") : tag_next);
+      cur->recs.push_back(rec_next);
     }
     tag_next.clear();
+    rec_next.clear();
     cur->launches += launches;
   }
   int emit_gemm(const GemmDesc& d, const float* rowvec_table = nullptr, int rowvec_stride = 0) {
@@ -170,6 +205,7 @@ struct Engine {
                     d.mode, L->bn, L->nsub, L->tr, d.b_batched ? " batched" : "");
       tag_next = buf;
     }
+    rec_next = gemm_record(d, *L, rowvec_table != nullptr);
     emit([L, rowvec_table, rowvec_stride](cudaStream_t st, int step) {
       if (rowvec_table) {
         GemmLaunch l = *L;
@@ -192,6 +228,7 @@ struct Engine {
     const int pad = kind == 2 ? 2 : 1;
     T xp = tmp(x.B, x.H + 2 * pad, x.W + 2 * pad, x.C);
     tag_next = "wrap pad (tiled)";
+    rec_next = wrap_pad_record(x.ld * 2, x.B, x.H, x.W, x.C * 2, pad);
     emit([=](cudaStream_t st, int) { return wrap_pad(x.p, x.ld * 2, x.B, x.H, x.W, x.C * 2, pad, xp.p, st); });
     const int oh = kind == 2 ? xp.H / 2 : (kind == 3 ? xp.H * 2 : xp.H), ow = kind == 2 ? xp.W / 2 : (kind == 3 ? xp.W * 2 : xp.W);
     const int crop = kind == 3 ? 2 : 1;
@@ -200,20 +237,31 @@ struct Engine {
     const T r = resid ? *resid : T{};
     const bool has_r = resid != nullptr;
     tag_next = "crop (tiled)";
+    rec_next = crop_record(out.B, out.H, out.W, N * 2, crop, has_r, r.ld, out.ld * 2);
     emit([=](cudaStream_t st, int) {
       return crop_interior(yp.p, out.B, out.H, out.W, N * 2, crop, has_r ? r.p : nullptr, r.ld, out.p, out.ld * 2, st);
     });
     return 0;
   }
   // the 4-channel edge convs of both nets (CUDA-core kernels) in tiled mode: same pad / run / crop scheme
+  static std::string conv_in_record(const T& x, int n, const T& o) {
+    return strf("conv_in_small\tldx=%lld\tB=%d\tH=%d\tW=%d\tCin=%d\tN=%d\tldy=%lld", ll(x.ld), x.B, x.H, x.W, x.C, n, ll(o.ld));
+  }
+  static std::string conv_out_record(const T& x, int oc, bool f32, bool u8) {
+    return strf("conv_out_small\tldx=%lld\tB=%d\tH=%d\tW=%d\tC=%d\tnout=%d\tf32=%d\tu8=%d", ll(x.ld), x.B, x.H, x.W, x.C, oc,
+                int(f32), int(u8));
+  }
   int conv_in_edge(const T& xin, const __half* w, const float* b, int n, const T& o) {
     if (!tiled) {
+      rec_next = conv_in_record(xin, n, o);
       emit([=](cudaStream_t st, int) { return conv_in_small(xin.p, xin.ld, xin.B, xin.H, xin.W, xin.C, w, b, n, o.p, o.ld, st); });
       return 0;
     }
     Scope scope(this);
     T xp = tmp(xin.B, xin.H + 2, xin.W + 2, xin.C);
     T yp = tmp(xin.B, xin.H + 2, xin.W + 2, n);
+    rec_next = wrap_pad_record(xin.ld * 2, xin.B, xin.H, xin.W, xin.C * 2, 1) + "\n" + conv_in_record(xp, n, yp) + "\n" +
+               crop_record(o.B, o.H, o.W, n * 2, 1, false, 0, o.ld * 2);
     emit([=](cudaStream_t st, int) {
       if (int e = wrap_pad(xin.p, xin.ld * 2, xin.B, xin.H, xin.W, xin.C * 2, 1, xp.p, st)) return e;
       if (int e = conv_in_small(xp.p, xp.ld, xp.B, xp.H, xp.W, xp.C, w, b, n, yp.p, yp.ld, st)) return e;
@@ -221,8 +269,11 @@ struct Engine {
     }, 3);
     return 0;
   }
-  int conv_out_edge(const T& n, const __half* w, const float* b, int oc, float* out_f32, uint8_t* out_u8) {
+  // frames: the op also writes uint8 frames (the VAE; the UNet writes fp32 eps only).  It sizes the launch count, which the
+  // dry run measures with null output pointers.
+  int conv_out_edge(const T& n, const __half* w, const float* b, int oc, float* out_f32, uint8_t* out_u8, bool frames) {
     if (!tiled) {
+      rec_next = conv_out_record(n, oc, out_f32 != nullptr, out_u8 != nullptr);
       emit([=](cudaStream_t st, int) { return conv_out_small(n.p, n.ld, n.B, n.H, n.W, n.C, w, b, oc, out_f32, out_u8, st); });
       return 0;
     }
@@ -230,7 +281,10 @@ struct Engine {
     T xp = tmp(n.B, n.H + 2, n.W + 2, n.C);
     const size_t pp = static_cast<size_t>(n.B) * (n.H + 2) * (n.W + 2);
     float* f32p = static_cast<float*>(scratch.take(pp * oc * 4));
-    uint8_t* u8p = out_u8 ? static_cast<uint8_t*>(scratch.take(pp * oc)) : nullptr;
+    uint8_t* u8p = frames ? static_cast<uint8_t*>(scratch.take(pp * oc)) : nullptr;
+    rec_next = wrap_pad_record(n.ld * 2, n.B, n.H, n.W, n.C * 2, 1) + "\n" + conv_out_record(xp, oc, true, out_u8 != nullptr);
+    if (out_f32) rec_next += "\n" + crop_record(n.B, n.H, n.W, oc * 4, 1, false, 0, oc * 4);
+    if (out_u8) rec_next += "\n" + crop_record(n.B, n.H, n.W, oc, 1, false, 0, oc);
     emit([=](cudaStream_t st, int) {
       if (int e = wrap_pad(n.p, n.ld * 2, n.B, n.H, n.W, n.C * 2, 1, xp.p, st)) return e;
       if (int e = conv_out_small(xp.p, xp.ld, xp.B, xp.H, xp.W, xp.C, w, b, oc, f32p, u8p, st)) return e;
@@ -238,7 +292,7 @@ struct Engine {
         if (int e = crop_interior(f32p, n.B, n.H, n.W, oc * 4, 1, nullptr, 0, out_f32, oc * 4, st)) return e;
       if (out_u8) return crop_interior(u8p, n.B, n.H, n.W, oc, 1, nullptr, 0, out_u8, oc, st);
       return 0;
-    }, 4);
+    }, frames ? 4 : 3);
     return 0;
   }
   int conv_zero_pad(const T& x, const __half* w, const float* bias, int N, int kind, const T& out, const T* resid = nullptr,
@@ -276,6 +330,8 @@ struct Engine {
     const int G = cfg_groups;
     float2* ws = gn_ws;
     tag_next = "groupnorm C" + std::to_string(x.C) + " " + std::to_string(x.B) + "x" + std::to_string(x.H) + "x" + std::to_string(x.W);
+    rec_next = strf("groupnorm\tB=%d\tP=%lld\tC=%d\tG=%d\tldx=%lld\tldy=%lld\tsilu=%d\teps=%.9g", x.B,
+                    ll(static_cast<int64_t>(x.H) * x.W), x.C, G, ll(x.ld), ll(out.ld), silu, static_cast<double>(eps));
     emit([=](cudaStream_t st, int) {
       return groupnorm(x.p, x.ld, x.B, static_cast<int64_t>(x.H) * x.W, x.C, G, g, b, eps, silu, out.p, out.ld, ws, st);
     }, groupnorm_launches());
@@ -284,6 +340,7 @@ struct Engine {
     const float* g = vec(name + ".weight", x.C);
     const float* b = vec(name + ".bias", x.C);
     tag_next = "layernorm C" + std::to_string(x.C) + " rows" + std::to_string(x.pixels());
+    rec_next = strf("layernorm\trows=%lld\tC=%d\tldx=%lld\tldy=%lld\teps=%.9g", ll(x.pixels()), x.C, ll(x.ld), ll(out.ld), 1e-5);
     emit([=](cudaStream_t st, int) { return layernorm(x.p, x.ld, x.pixels(), x.C, g, b, 1e-5f, out.p, out.ld, st); });
   }
   int cfg_groups = 32;
@@ -305,6 +362,11 @@ struct Engine {
       if (int e = plan_attention(a, L.get())) return e;
       tag_next = "attention d" + std::to_string(d) + " B" + std::to_string(Bq) + " h" + std::to_string(heads) + " Nq" +
                  std::to_string(Nq) + " Nk" + std::to_string(Nk);
+      int plan[5];
+      attention_plan_info(*L, plan);
+      rec_next = strf("attention\tB=%d\tNq=%d\tNk=%d\theads=%d\td=%d\tq_ld=%lld\tk_ld=%lld\tvt_ld=%lld\tout_ld=%lld\tvariant=%d\t"
+                      "gx=%d\tgy=%d\tgz=%d", Bq, Nq, Nk, heads, d, ll(q_ld), ll(k_ld), ll(vt_ld), ll(out.ld), plan[0], plan[2],
+                      plan[3], plan[4]);
       emit([L](cudaStream_t st, int) { return launch_attention(*L, st); });
       return 0;
     }
@@ -326,6 +388,7 @@ struct Engine {
       if (int e = emit_gemm(g)) return e;
       __half* Sp = S;
       const int64_t rows = static_cast<int64_t>(nb) * heads * Nq;
+      rec_next = strf("softmax_rows\tld=%lld\trows=%lld\tn=%d", ll(Nkp), ll(rows), Nk);
       emit([=](cudaStream_t st, int) { return softmax_rows(Sp, Nkp, rows, Nk, st); });
       GemmDesc h;
       h.A = S; h.C = Nk; h.W = Nq; h.H = heads; h.B = nb;
@@ -587,7 +650,7 @@ struct Engine {
       float* e_out = eps;
       const int oc = cfg.out_channels;
       tag_next = "conv_out C->4 (CUDA cores)";
-      if (int e = conv_out_edge(n, w, b, oc, e_out, nullptr)) return e;
+      if (int e = conv_out_edge(n, w, b, oc, e_out, nullptr, false)) return e;
     }
     return 0;
   }
@@ -607,6 +670,7 @@ struct Engine {
       const float* xs = x;
       const float inv = 1.f / cfg.vae_scaling_factor;
       tag_next = "vae_in (scale + post_quant 1x1)";
+      rec_next = strf("vae_in\tF=%d\tC=%d\tH=%d\tW=%d\tinv_scale=%.9g", F, lc, H0, W0, static_cast<double>(inv));
       emit([=](cudaStream_t st, int) { return vae_in(xs, inv, w, b, F, lc, H0, W0, z.p, st); });
     }
     T h = pingpong(F, H0, W0, ctop);
@@ -684,7 +748,7 @@ struct Engine {
       float* of = out_img_f32;
       const int oc = cfg.vae_out_channels;
       tag_next = "vae conv_out C->3 + uint8 (CUDA cores)";
-      if (int e = conv_out_edge(n, w, b, oc, of, o8)) return e;
+      if (int e = conv_out_edge(n, w, b, oc, of, o8, true)) return e;
     }
     return 0;
   }
@@ -997,6 +1061,27 @@ int sdw_engine_launches(const sdw_engine* e, int* prologue, int* unet, int* vae)
 }
 
 // ---- debug / parity entry points -------------------------------------------------------------------
+// tooling: the recorded arguments of every op of the UNet and VAE lists (written at bind time; nothing is launched)
+int sdw_engine_debug_ops(const sdw_engine* e, const char* path) {
+  const Engine* E = reinterpret_cast<const Engine*>(e);
+  SDW_REQUIRE(E && path && !E->dry, "engine not bound");
+  FILE* f = std::fopen(path, "w");
+  SDW_REQUIRE(f, "cannot open the op list file");
+  const std::pair<const char*, const OpList*> sections[2] = {{"unet", &E->unet_ops}, {"vae", &E->vae_ops}};
+  for (const auto& s : sections)
+    for (size_t i = 0; i < s.second->recs.size(); ++i) {
+      const std::string& r = s.second->recs[i];
+      for (size_t a = 0; a <= r.size();) {
+        size_t b = r.find('\n', a);
+        if (b == std::string::npos) b = r.size();
+        std::fprintf(f, "%s\t%zu\t%s\n", s.first, i, r.substr(a, b - a).c_str());
+        a = b + 1;
+      }
+    }
+  std::fclose(f);
+  return 0;
+}
+
 // tooling: time every op of one UNet forward (step 0) and of the VAE decode with CUDA events, after one untimed pass;
 // writes "section<TAB>index<TAB>microseconds<TAB>tag" lines.  The engine must be bound and have sampled once.
 int sdw_engine_debug_profile(sdw_engine* e, const char* path, void* stream) {

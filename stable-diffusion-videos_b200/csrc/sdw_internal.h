@@ -321,10 +321,12 @@ using OpFn = std::function<int(cudaStream_t, int /*step*/)>;
 struct OpList {
   std::vector<OpFn> ops;
   std::vector<std::string> tags;
+  std::vector<std::string> recs;  // sampler engine: each op's "kind<TAB>key=value..." line(s) (sdw_engine_debug_ops)
   int launches = 0;
   void clear() {
     ops.clear();
     tags.clear();
+    recs.clear();
     launches = 0;
   }
   int run(cudaStream_t st, int step) const;
