@@ -121,9 +121,9 @@ int sdw_engine_create(const sdw_engine_config* cfg, sdw_engine** out);
 void sdw_engine_destroy(sdw_engine* e);
 int sdw_engine_arena_bytes(const sdw_engine* e, uint64_t* bytes);
 int sdw_engine_bind(sdw_engine* e, void* arena, uint64_t bytes);
-/* The parameter table, the same for all three engines (sampler, CLIP tower, upsampler): param_info enumerates index
- * 0 .. num_params-1 in the engine's registration order (for this engine, not alphabetically: the key set is that of the
- * checkpoint).  load_param returns 1 without launching anything when the engine is not bound, the name is unknown or
+/* The parameter table, the same for all four engines (sampler, CLIP tower, upsampler, safety checker): param_info
+ * enumerates index 0 .. num_params-1 in the engine's registration order (for this engine, not alphabetically: the key
+ * set is that of the checkpoint).  load_param returns 1 without launching anything when the engine is not bound, the name is unknown or
  * numel differs, with a message naming the parameter.  missing_params counts the parameters not loaded yet and names
  * the first in `first_missing`; it returns -1 for a null engine. */
 int sdw_engine_num_params(const sdw_engine* e);

@@ -7,11 +7,14 @@
 // wgmma GEMM of sdw_gemm.cu (M = 77 B rows: one or two 128-row tiles), LayerNorm on sdw_norm.cu's kernel; the
 // 77 x 77 causal attention per head and the embedding gather are small CUDA-core kernels here (13 GFLOP per prompt: the
 // tower is a feed of the hot loop, not part of it).  State-dict names are transformers' `CLIPTextModel` keys.
+// The encoder layers (`ClipEncoder`) also make the safety checker's image tower (sdw_safety.cu), there not causal.
 #include "sdw_internal.h"
 #include "sdw_ptx.cuh"
 
 #include <cmath>
 #include <cstring>
+#include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -104,80 +107,142 @@ __global__ void clip_act_kernel(__half* __restrict__ x, int64_t n, int gelu_erf)
   x[i] = __float2half_rn(y);
 }
 
+static int clip_attention(const __half* qkv, int B, int P, int heads, __half* out, cudaStream_t st) {
+  clip_attn_kernel<96><<<dim3(heads, B), 128, 0, st>>>(qkv, P, heads * 64, out);
+  SDW_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+static int clip_act(__half* x, int64_t n, int gelu_erf, cudaStream_t st) {
+  clip_act_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(x, n, gelu_erf);
+  SDW_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// the encoder
+// ---------------------------------------------------------------------------------------------
+void ClipEncoder::layout(Arena& arena, ParamTable& params, const std::string& prefix, int n_layers, int H, int I) {
+  hidden = H;
+  intermediate = I;
+  layers.assign(n_layers, Layer{});
+  for (int i = 0; i < n_layers; ++i) {
+    Layer& L = layers[i];
+    const std::string p = prefix + std::to_string(i) + ".";
+    L.ln1_g = arena.take<float>(H); L.ln1_b = arena.take<float>(H);
+    L.ln2_g = arena.take<float>(H); L.ln2_b = arena.take<float>(H);
+    L.bqkv = arena.take<float>(3 * H); L.bo = arena.take<float>(H);
+    L.b1 = arena.take<float>(I); L.b2 = arena.take<float>(H);
+    L.wqkv = arena.take<__half>(static_cast<size_t>(3) * H * H);
+    L.wo = arena.take<__half>(static_cast<size_t>(H) * H);
+    L.w1 = arena.take<__half>(static_cast<size_t>(I) * H);
+    L.w2 = arena.take<__half>(static_cast<size_t>(H) * I);
+    params.add(p + "layer_norm1.weight", VEC, L.ln1_g, H); params.add(p + "layer_norm1.bias", VEC, L.ln1_b, H);
+    params.add(p + "layer_norm2.weight", VEC, L.ln2_g, H); params.add(p + "layer_norm2.bias", VEC, L.ln2_b, H);
+    const char* qkvn[3] = {"q_proj", "k_proj", "v_proj"};
+    for (int k = 0; k < 3; ++k) {
+      params.add(p + "self_attn." + qkvn[k] + ".weight", PACKED, L.wqkv ? L.wqkv + static_cast<size_t>(k) * H * H : nullptr,
+                 static_cast<int64_t>(H) * H, H, H);
+      params.add(p + "self_attn." + qkvn[k] + ".bias", VEC, L.bqkv ? L.bqkv + k * H : nullptr, H);
+    }
+    params.add(p + "self_attn.out_proj.weight", PACKED, L.wo, static_cast<int64_t>(H) * H, H, H);
+    params.add(p + "self_attn.out_proj.bias", VEC, L.bo, H);
+    params.add(p + "mlp.fc1.weight", PACKED, L.w1, static_cast<int64_t>(I) * H, I, H);
+    params.add(p + "mlp.fc1.bias", VEC, L.b1, I);
+    params.add(p + "mlp.fc2.weight", PACKED, L.w2, static_cast<int64_t>(H) * I, H, I);
+    params.add(p + "mlp.fc2.bias", VEC, L.b2, H);
+  }
+}
+
+// out[T][N] = a[T][K] w^T + bias (+ resid)
+static GemmDesc linear_desc(const __half* a, int64_t T, int K, const __half* w, int N, const float* bias,
+                            const __half* resid, __half* out) {
+  GemmDesc d;
+  d.A = a; d.C = K; d.W = static_cast<int>(T); d.H = 1; d.B = 1; d.sW = K;
+  d.Wt = w; d.N = N; d.bias = bias; d.resid = resid; d.out = out; d.ldc = N;
+  return d;
+}
+
+int ClipEncoder::emit(OpList& ops, int B, int P, float eps, int gelu_erf, bool causal, const Buffers& b) const {
+  const int H = hidden, I = intermediate, heads = H / 64;
+  const int64_t T = static_cast<int64_t>(B) * P;
+  __half *x = b.x, *y = b.y, *h = b.h, *ff = b.ff, *qkv = b.qkv;
+  for (size_t i = 0; i < layers.size(); ++i) {
+    const Layer& L = layers[i];
+    const std::string p = "layer " + std::to_string(i) + " ";
+    ops.add(p + "ln1", [=](cudaStream_t st, int) { return layernorm(x, H, T, H, L.ln1_g, L.ln1_b, eps, h, H, st); });
+    GemmDesc g = linear_desc(h, T, H, L.wqkv, 3 * H, L.bqkv, nullptr, qkv);
+    if (causal) {
+      if (int e = ops.add_gemm(g, p + "qkv")) return e;
+      ops.add(p + "attention", [=](cudaStream_t st, int) { return clip_attention(qkv, B, P, heads, h, st); });
+    } else {
+      g.ldc = 2 * H;
+      g.mode = GEMM_QKV_VT;
+      g.vt_col0 = 2 * H; g.vt_d = 64; g.vt_heads = heads; g.vt_ntok = P; g.vt = b.vt; g.vt_ld = b.vt_ld;
+      if (int e = ops.add_gemm(g, p + "qkv + V^T")) return e;
+      AttnDesc ad;
+      ad.q = qkv; ad.q_ld = 2 * H; ad.k = qkv + H; ad.k_ld = 2 * H; ad.vt = b.vt; ad.vt_ld = b.vt_ld;
+      ad.B = B; ad.Nq = P; ad.Nk = P; ad.heads = heads; ad.d = 64;
+      ad.out = h; ad.out_ld = H;
+      auto AL = std::make_shared<AttnLaunch>();
+      if (int e = plan_attention(ad, AL.get())) return e;
+      ops.add(p + "attention", [AL](cudaStream_t st, int) { return launch_attention(*AL, st); });
+    }
+    if (int e = ops.add_gemm(linear_desc(h, T, H, L.wo, H, L.bo, x, y), p + "out_proj + x")) return e;
+    std::swap(x, y);
+    ops.add(p + "ln2", [=](cudaStream_t st, int) { return layernorm(x, H, T, H, L.ln2_g, L.ln2_b, eps, h, H, st); });
+    if (int e = ops.add_gemm(linear_desc(h, T, H, L.w1, I, L.b1, nullptr, ff), p + "fc1")) return e;
+    ops.add(p + "act", [=](cudaStream_t st, int) { return clip_act(ff, T * I, gelu_erf, st); });
+    if (int e = ops.add_gemm(linear_desc(ff, T, I, L.w2, H, L.b2, x, y), p + "fc2 + x")) return e;
+    std::swap(x, y);
+  }
+  return 0;
+}
+
 // ---------------------------------------------------------------------------------------------
 // engine
 // ---------------------------------------------------------------------------------------------
-struct ClipLayer {
-  float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bo, *b1, *b2;
-  __half *wqkv, *wo, *w1, *w2;
-};
-
 struct ClipEngine {
   sdw_clip_config cfg;
   Arena arena{256};
   size_t cap = 0;
   ParamTable params;
-  std::vector<ClipLayer> layers;
+  ClipEncoder enc;
   __half *tok = nullptr, *pos = nullptr;
   float *lnf_g = nullptr, *lnf_b = nullptr;
   __half *x0 = nullptr, *x1 = nullptr, *h = nullptr, *qkv = nullptr, *ff = nullptr;
-  int32_t* ids = nullptr;
+  std::map<int, OpList> towers;  // encoder ops per batch size
 
   void layout(void* base) {
     const sdw_clip_config& c = cfg;
     const int H = c.hidden, I = c.intermediate;
     arena.reset(base);
     params.clear(base != nullptr);
-    layers.assign(c.layers, ClipLayer{});
+    towers.clear();
     tok = arena.take<__half>(static_cast<size_t>(c.vocab) * H);
     pos = arena.take<__half>(static_cast<size_t>(c.max_positions) * H);
     params.add("text_model.embeddings.token_embedding.weight", RAW, tok, static_cast<int64_t>(c.vocab) * H);
     params.add("text_model.embeddings.position_embedding.weight", RAW, pos, static_cast<int64_t>(c.max_positions) * H);
-    for (int i = 0; i < c.layers; ++i) {
-      ClipLayer& L = layers[i];
-      const std::string p = "text_model.encoder.layers." + std::to_string(i) + ".";
-      L.ln1_g = arena.take<float>(H); L.ln1_b = arena.take<float>(H);
-      L.ln2_g = arena.take<float>(H); L.ln2_b = arena.take<float>(H);
-      L.bqkv = arena.take<float>(3 * H); L.bo = arena.take<float>(H);
-      L.b1 = arena.take<float>(I); L.b2 = arena.take<float>(H);
-      L.wqkv = arena.take<__half>(static_cast<size_t>(3) * H * H);
-      L.wo = arena.take<__half>(static_cast<size_t>(H) * H);
-      L.w1 = arena.take<__half>(static_cast<size_t>(I) * H);
-      L.w2 = arena.take<__half>(static_cast<size_t>(H) * I);
-      params.add(p + "layer_norm1.weight", VEC, L.ln1_g, H); params.add(p + "layer_norm1.bias", VEC, L.ln1_b, H);
-      params.add(p + "layer_norm2.weight", VEC, L.ln2_g, H); params.add(p + "layer_norm2.bias", VEC, L.ln2_b, H);
-      const char* qkvn[3] = {"q_proj", "k_proj", "v_proj"};
-      for (int k = 0; k < 3; ++k) {
-        params.add(p + "self_attn." + qkvn[k] + ".weight", PACKED, L.wqkv ? L.wqkv + static_cast<size_t>(k) * H * H : nullptr,
-                   static_cast<int64_t>(H) * H, H, H);
-        params.add(p + "self_attn." + qkvn[k] + ".bias", VEC, L.bqkv ? L.bqkv + k * H : nullptr, H);
-      }
-      params.add(p + "self_attn.out_proj.weight", PACKED, L.wo, static_cast<int64_t>(H) * H, H, H);
-      params.add(p + "self_attn.out_proj.bias", VEC, L.bo, H);
-      params.add(p + "mlp.fc1.weight", PACKED, L.w1, static_cast<int64_t>(I) * H, I, H);
-      params.add(p + "mlp.fc1.bias", VEC, L.b1, I);
-      params.add(p + "mlp.fc2.weight", PACKED, L.w2, static_cast<int64_t>(H) * I, H, I);
-      params.add(p + "mlp.fc2.bias", VEC, L.b2, H);
-    }
+    enc.layout(arena, params, "text_model.encoder.layers.", c.layers, H, I);
     lnf_g = arena.take<float>(H); lnf_b = arena.take<float>(H);
     params.add("text_model.final_layer_norm.weight", VEC, lnf_g, H);
     params.add("text_model.final_layer_norm.bias", VEC, lnf_b, H);
     const size_t T = static_cast<size_t>(c.max_batch) * c.max_positions;
     x0 = arena.take<__half>(T * H); x1 = arena.take<__half>(T * H); h = arena.take<__half>(T * H);
     qkv = arena.take<__half>(T * 3 * H); ff = arena.take<__half>(T * I);
-    ids = arena.take<int32_t>(T);
+  }
+
+  // the encoder of B prompts, from the embeddings in x0 to its result in x0; planned on first use
+  const OpList* tower(int B) {
+    auto it = towers.find(B);
+    if (it != towers.end()) return &it->second;
+    OpList ops;
+    ClipEncoder::Buffers b;
+    b.x = x0; b.y = x1; b.h = h; b.ff = ff; b.qkv = qkv;
+    if (enc.emit(ops, B, cfg.max_positions, cfg.eps, cfg.act_gelu_erf, true, b)) return nullptr;
+    return &(towers[B] = std::move(ops));
   }
 };
-
-static int clip_linear(const __half* a, int64_t T, int K, const __half* w, int N, const float* bias, const __half* resid,
-                       __half* out, cudaStream_t st) {
-  GemmDesc d;
-  d.A = a; d.C = K; d.W = static_cast<int>(T); d.H = 1; d.B = 1; d.sW = K;
-  d.Wt = w; d.N = N; d.bias = bias; d.resid = resid; d.ldr = N; d.out = out; d.ldc = N;
-  GemmLaunch L;
-  if (int e = plan_gemm(d, &L)) return e;
-  return launch_gemm(L, st);
-}
 
 }  // namespace sdw
 
@@ -239,28 +304,16 @@ int sdw_clip_forward(sdw_clip* e, const int32_t* ids, int B, void* out_f16, void
   const sdw_clip_config& c = E->cfg;
   SDW_REQUIRE(B >= 1 && B <= c.max_batch, "batch exceeds max_batch");
   SDW_REQUIRE(E->params.missing(nullptr) == 0, "CLIP parameters not loaded");
+  const OpList* t = E->tower(B);
+  if (!t) return 1;
+  // no CUDA graph: the caller's stream may be the legacy default stream, which cannot be captured
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int P = c.max_positions, H = c.hidden, I = c.intermediate;
+  const int P = c.max_positions, H = c.hidden;
   const int64_t T = static_cast<int64_t>(B) * P;
   clip_embed_kernel<<<static_cast<unsigned>(T), 128, 0, st>>>(ids, E->tok, E->pos, P, H, c.vocab, E->x0);
   SDW_CUDA_OK(cudaGetLastError());
-  __half *x = E->x0, *y = E->x1;
-  for (int i = 0; i < c.layers; ++i) {
-    const ClipLayer& L = E->layers[i];
-    if (int rc = layernorm(x, H, T, H, L.ln1_g, L.ln1_b, c.eps, E->h, H, st)) return rc;
-    if (int rc = clip_linear(E->h, T, H, L.wqkv, 3 * H, L.bqkv, nullptr, E->qkv, st)) return rc;
-    clip_attn_kernel<96><<<dim3(c.heads, B), 128, 0, st>>>(E->qkv, P, H, E->h);
-    SDW_CUDA_OK(cudaGetLastError());
-    if (int rc = clip_linear(E->h, T, H, L.wo, H, L.bo, x, y, st)) return rc;
-    std::swap(x, y);
-    if (int rc = layernorm(x, H, T, H, L.ln2_g, L.ln2_b, c.eps, E->h, H, st)) return rc;
-    if (int rc = clip_linear(E->h, T, H, L.w1, I, L.b1, nullptr, E->ff, st)) return rc;
-    clip_act_kernel<<<static_cast<unsigned>((T * I + 255) / 256), 256, 0, st>>>(E->ff, T * I, c.act_gelu_erf);
-    SDW_CUDA_OK(cudaGetLastError());
-    if (int rc = clip_linear(E->ff, T, I, L.w2, H, L.b2, x, y, st)) return rc;
-    std::swap(x, y);
-  }
-  return layernorm(x, H, T, H, E->lnf_g, E->lnf_b, c.eps, static_cast<__half*>(out_f16), H, st);
+  if (int rc = t->run(st, 0)) return rc;
+  return layernorm(E->x0, H, T, H, E->lnf_g, E->lnf_b, c.eps, static_cast<__half*>(out_f16), H, st);
 }
 
 // the tower's three kernels on their own (tests / tooling)
@@ -280,20 +333,15 @@ int sdw_clip_attention(const void* qkv, int B, int P, int heads, void* out, void
   SDW_REQUIRE(qkv && out, "null");
   SDW_REQUIRE(P >= 1 && P <= 96, "CLIP attention: 1 <= P <= 96 (the kernel stages K and V of 96 positions)");
   SDW_REQUIRE(B >= 1 && B <= 65535 && heads >= 1 && heads <= 65535, "CLIP attention: bad B / heads");
-  clip_attn_kernel<96><<<dim3(heads, B), 128, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const __half*>(qkv), P, heads * 64, static_cast<__half*>(out));
-  SDW_CUDA_OK(cudaGetLastError());
-  return 0;
+  return clip_attention(static_cast<const __half*>(qkv), B, P, heads, static_cast<__half*>(out),
+                        static_cast<cudaStream_t>(stream));
 }
 
 int sdw_clip_act(void* x, int64_t n, int gelu_erf, void* stream) {
   SDW_REQUIRE(x && n >= 0 && (gelu_erf == 0 || gelu_erf == 1), "CLIP activation: null x, n < 0 or bad activation");
   SDW_REQUIRE(n <= int64_t(1) << 38, "CLIP activation: n too large for one launch");
   if (n == 0) return 0;
-  clip_act_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<__half*>(x), n, gelu_erf);
-  SDW_CUDA_OK(cudaGetLastError());
-  return 0;
+  return clip_act(static_cast<__half*>(x), n, gelu_erf, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

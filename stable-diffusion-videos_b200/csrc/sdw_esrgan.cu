@@ -28,7 +28,6 @@
 #include <algorithm>
 #include <cstdio>
 #include <functional>
-#include <memory>
 #include <string>
 #include <vector>
 
@@ -129,17 +128,6 @@ struct EsrEngine {
     d.Wt = Wt; d.N = N; d.bias = b; d.out = out; d.ldc = ldc; d.act = act;
     return d;
   }
-  int add(const GemmDesc& d, const std::string& tag) {
-    auto L = std::make_shared<GemmLaunch>();
-    if (int e = plan_gemm(d, L.get())) {
-      set_error(tag + ": " + last_error());
-      return e;
-    }
-    gemms.ops.push_back([L](cudaStream_t st, int) { return launch_gemm(*L, st); });
-    gemms.tags.push_back(tag);
-    gemms.launches += 1;
-    return 0;
-  }
   int build_ops() {
     gemms.clear();
     const int nf = cfg.num_feat, gc = cfg.num_grow_ch, cat = nf + 4 * gc;
@@ -156,8 +144,8 @@ struct EsrEngine {
           GemmDesc d = desc(in, nf + gc * k, cat, W, H, c.w, gc, c.b, in + nf + gc * k, cat, 2);
           d.bn = 32;
           d.ver = 1;
-          if (int e = add(d, pre + "conv" + std::to_string(k + 1) + " " + std::to_string(nf + gc * k) + "->32 lrelu"))
-            return e;
+          const std::string tag = pre + "conv" + std::to_string(k + 1) + " " + std::to_string(nf + gc * k) + "->32 lrelu";
+          if (int e = gemms.add_gemm(d, tag)) return e;
         }
         const EsrConv& c5 = body[(i * 3 + r) * 5 + 4];
         GemmDesc d = desc(in, cat, cat, W, H, c5.w, nf, c5.b, bufs[r + 1], cat, 0);
@@ -170,7 +158,7 @@ struct EsrEngine {
           d.res_scale = 0.2f;
           d.resid2 = X[cur];
         }
-        if (int e = add(d, pre + "conv5 192->64" + (r < 2 ? " x0.2 + x" : " x0.04 + 0.2 r + x_rrdb"))) return e;
+        if (int e = gemms.add_gemm(d, pre + "conv5 192->64" + (r < 2 ? " x0.2 + x" : " x0.04 + 0.2 r + x_rrdb"))) return e;
       }
       cur = nxt;
     }
@@ -178,7 +166,7 @@ struct EsrEngine {
       GemmDesc d = desc(X[cur], nf, cat, W, H, body_conv.w, nf, body_conv.b, t, nf, 0);
       d.resid = X[0];
       d.ldr = cat;
-      if (int e = add(d, "conv_body + feat")) return e;
+      if (int e = gemms.add_gemm(d, "conv_body + feat")) return e;
     }
     const __half* src[2] = {t, u1};
     __half* dst[2] = {u1, u2};
@@ -191,11 +179,11 @@ struct EsrEngine {
         d.conv = 3;
         d.up_px = px;
         d.up_py = py;
-        if (int e = add(d, std::string("conv_up") + char('1' + s) + " parity " + char('0' + py) + char('0' + px) + " lrelu"))
-          return e;
+        const std::string tag = std::string("conv_up") + char('1' + s) + " parity " + char('0' + py) + char('0' + px) + " lrelu";
+        if (int e = gemms.add_gemm(d, tag)) return e;
       }
     GemmDesc d = desc(u2, nf, nf, 4 * W, 4 * H, hr.w, nf, hr.b, h, nf, 2);
-    return add(d, "conv_hr lrelu");
+    return gemms.add_gemm(d, "conv_hr lrelu");
   }
 };
 
@@ -301,18 +289,15 @@ int sdw_upsampler_debug_profile(sdw_upsampler* e, const char* path, void* stream
   const uint8_t* in_scratch = E->Q;  // dead while conv_first runs
   uint8_t* out_scratch = E->P;       // dead while conv_last runs
   OpList ops;
-  ops.ops.push_back([=](cudaStream_t st, int) {
+  ops.add("conv_first u8 3->64 (CUDA cores)", [=](cudaStream_t st, int) {
     return conv_first_u8(in_scratch, c.frames, c.in_h, c.in_w, E->first.w, E->first.b, c.num_feat, E->X[0],
                          c.num_feat + 4 * c.num_grow_ch, st);
   });
-  ops.tags.push_back("conv_first u8 3->64 (CUDA cores)");
-  ops.ops.insert(ops.ops.end(), E->gemms.ops.begin(), E->gemms.ops.end());
-  ops.tags.insert(ops.tags.end(), E->gemms.tags.begin(), E->gemms.tags.end());
-  ops.ops.push_back([=](cudaStream_t st, int) {
+  ops.append(E->gemms);
+  ops.add("conv_last 64->3 + uint8 (CUDA cores)", [=](cudaStream_t st, int) {
     return conv_out_small(E->h, c.num_feat, c.frames, 4 * c.in_h, 4 * c.in_w, c.num_feat, E->last.w, E->last.b, 3,
                           nullptr, out_scratch, st, 1);
   });
-  ops.tags.push_back("conv_last 64->3 + uint8 (CUDA cores)");
   FILE* f = std::fopen(path, "w");
   SDW_REQUIRE(f, "cannot open the profile file");
   int rc = profile_ops(f, "upsampler", ops, static_cast<cudaStream_t>(stream), 0);

@@ -330,6 +330,10 @@ struct OpList {
     launches = 0;
   }
   int run(cudaStream_t st, int step) const;
+  void add(const std::string& tag, OpFn f);  // one op of one launch
+  // plans `d` now and adds its launch; a plan error is reported as "tag: message"
+  int add_gemm(const GemmDesc& d, const std::string& tag);
+  void append(const OpList& o);
 };
 
 // one instantiated CUDA graph of `body`, re-captured when the key changes
@@ -346,5 +350,30 @@ struct GraphCache {
 
 // tooling: one untimed pass of `ops`, then CUDA events around every op; writes "section<TAB>index<TAB>us<TAB>tag" lines
 int profile_ops(FILE* f, const char* section, const OpList& ops, cudaStream_t st, int step);
+
+// ---------------------------------------------------------------------------
+// the pre-LN CLIP transformer encoder (sdw_clip.cu), shared by the text tower and the safety checker's image tower
+// ---------------------------------------------------------------------------
+struct ClipEncoder {
+  struct Layer {
+    float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bo, *b1, *b2;
+    __half *wqkv, *wo, *w1, *w2;  // q | k | v rows packed into one weight
+  };
+  struct Buffers {         // activations of B sequences of P tokens, T = B P rows
+    __half *x, *y;         // residual stream [T][hidden]: x holds the input, y is the other half of the ping-pong
+    __half *h, *ff;        // LayerNorm and attention outputs [T][hidden]; MLP [T][intermediate]
+    __half* qkv;           // causal: [T][3 hidden]; otherwise q | k [T][2 hidden]
+    __half* vt = nullptr;  // not causal: V^T [B][heads][64][vt_ld], written by the QKV GEMM's epilogue
+    int64_t vt_ld = 0;
+  };
+  int hidden = 0, intermediate = 0;
+  std::vector<Layer> layers;
+  // takes each layer's arena slots and registers `prefix`{i}.layer_norm1.weight ... mlp.fc2.bias
+  void layout(Arena& arena, ParamTable& params, const std::string& prefix, int n_layers, int hidden, int intermediate);
+  // Appends the layers' ops (64-wide heads; gelu_erf: 0 quick-GELU, 1 erf GELU).  Causal: a plain QKV GEMM and
+  // clip_attn_kernel; otherwise the QKV GEMM with the V^T epilogue and the fused attention.  The result ends in b.x
+  // (each layer adds attention into y, then its MLP back into x).  Returns a plan error with its message set, else 0.
+  int emit(OpList& ops, int B, int P, float eps, int gelu_erf, bool causal, const Buffers& b) const;
+};
 
 }  // namespace sdw

@@ -1,8 +1,9 @@
-// sdw_model.cu — host scaffolding shared by the three engines (sampler, CLIP text tower, upsampler): the arena bump
-// allocator, the parameter table and its load dispatch, op lists, CUDA-graph replay and the per-op profile.
+// sdw_model.cu — host scaffolding shared by the four engines (sampler, CLIP text tower, upsampler, safety checker): the
+// arena bump allocator, the parameter table and its load dispatch, op lists, CUDA-graph replay and the per-op profile.
 #include "sdw_internal.h"
 
 #include <algorithm>
+#include <memory>
 
 namespace sdw {
 
@@ -92,6 +93,28 @@ int OpList::run(cudaStream_t st, int step) const {
   for (const OpFn& f : ops)
     if (int rc = f(st, step)) return rc;
   return 0;
+}
+
+void OpList::add(const std::string& tag, OpFn f) {
+  ops.push_back(std::move(f));
+  tags.push_back(tag);
+  launches += 1;
+}
+
+int OpList::add_gemm(const GemmDesc& d, const std::string& tag) {
+  auto L = std::make_shared<GemmLaunch>();
+  if (int e = plan_gemm(d, L.get())) {
+    set_error(tag + ": " + last_error());
+    return e;
+  }
+  add(tag, [L](cudaStream_t st, int) { return launch_gemm(*L, st); });
+  return 0;
+}
+
+void OpList::append(const OpList& o) {
+  ops.insert(ops.end(), o.ops.begin(), o.ops.end());
+  tags.insert(tags.end(), o.tags.begin(), o.tags.end());
+  launches += o.launches;
 }
 
 void GraphCache::reset() {

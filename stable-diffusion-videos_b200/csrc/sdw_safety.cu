@@ -6,9 +6,9 @@
 // Preprocessing is bit-exact with Pillow at the uint8 stage: the host builds Pillow's coefficient tables
 // (precompute_coeffs + normalize_coeffs_8bpc, 22-bit fixed point) and two kernels run its horizontal-then-vertical
 // passes, the vertical one only for the 224 x 224 pixels the crop keeps.  The patch conv is a GEMM whose A rows are
-// written by the normalisation kernel; the transformer reuses LayerNorm, the wgmma GEMM (QKV with the V^T epilogue) and
-// the fused attention of the sampler, and the CLIP tower's activation kernel.  State-dict names are diffusers'
-// `StableDiffusionSafetyChecker` keys.
+// written by the normalisation kernel; the transformer layers are the CLIP text tower's `ClipEncoder` (sdw_clip.cu)
+// without the causal mask: the QKV GEMM with the V^T epilogue and the sampler's fused attention.  State-dict names are
+// diffusers' `StableDiffusionSafetyChecker` keys.
 #include "sdw_internal.h"
 #include "sdw_ptx.cuh"
 
@@ -223,11 +223,6 @@ __global__ void __launch_bounds__(256) safety_score_kernel(const float* __restri
 // ---------------------------------------------------------------------------------------------
 // engine
 // ---------------------------------------------------------------------------------------------
-struct SafetyLayer {
-  float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *bqkv, *bo, *b1, *b2;
-  __half *wqkv, *wo, *w1, *w2;
-};
-
 struct SafetyTower {  // the transformer ops of one chunk size, replayed as a CUDA graph
   OpList ops;
   GraphCache graph;
@@ -238,7 +233,7 @@ struct SafetyEngine {
   Arena arena{256};
   size_t cap = 0;
   ParamTable params;
-  std::vector<SafetyLayer> layers;
+  ClipEncoder enc;
   int np = 0, ntok = 0, K = 0, Kp = 0;
   int64_t vt_ld = 0;
   __half *patch_w = nullptr, *cls = nullptr, *pos = nullptr, *proj_w = nullptr;
@@ -270,7 +265,6 @@ struct SafetyEngine {
     vt_ld = (ntok + 7) / 8 * 8;
     arena.reset(base);
     params.clear(base != nullptr);
-    layers.assign(c.layers, SafetyLayer{});
     towers.clear();
     const std::string vm = "vision_model.vision_model.";
     cls = arena.take<__half>(Hd);
@@ -282,32 +276,7 @@ struct SafetyEngine {
     pre_g = arena.take<float>(Hd); pre_b = arena.take<float>(Hd);
     params.add(vm + "pre_layrnorm.weight", VEC, pre_g, Hd);
     params.add(vm + "pre_layrnorm.bias", VEC, pre_b, Hd);
-    for (int i = 0; i < c.layers; ++i) {
-      SafetyLayer& L = layers[i];
-      const std::string p = vm + "encoder.layers." + std::to_string(i) + ".";
-      L.ln1_g = arena.take<float>(Hd); L.ln1_b = arena.take<float>(Hd);
-      L.ln2_g = arena.take<float>(Hd); L.ln2_b = arena.take<float>(Hd);
-      L.bqkv = arena.take<float>(3 * Hd); L.bo = arena.take<float>(Hd);
-      L.b1 = arena.take<float>(I); L.b2 = arena.take<float>(Hd);
-      L.wqkv = arena.take<__half>(static_cast<size_t>(3) * Hd * Hd);
-      L.wo = arena.take<__half>(static_cast<size_t>(Hd) * Hd);
-      L.w1 = arena.take<__half>(static_cast<size_t>(I) * Hd);
-      L.w2 = arena.take<__half>(static_cast<size_t>(Hd) * I);
-      params.add(p + "layer_norm1.weight", VEC, L.ln1_g, Hd); params.add(p + "layer_norm1.bias", VEC, L.ln1_b, Hd);
-      params.add(p + "layer_norm2.weight", VEC, L.ln2_g, Hd); params.add(p + "layer_norm2.bias", VEC, L.ln2_b, Hd);
-      const char* qkvn[3] = {"q_proj", "k_proj", "v_proj"};
-      for (int k = 0; k < 3; ++k) {
-        params.add(p + "self_attn." + qkvn[k] + ".weight", PACKED,
-                   L.wqkv ? L.wqkv + static_cast<size_t>(k) * Hd * Hd : nullptr, static_cast<int64_t>(Hd) * Hd, Hd, Hd);
-        params.add(p + "self_attn." + qkvn[k] + ".bias", VEC, L.bqkv ? L.bqkv + k * Hd : nullptr, Hd);
-      }
-      params.add(p + "self_attn.out_proj.weight", PACKED, L.wo, static_cast<int64_t>(Hd) * Hd, Hd, Hd);
-      params.add(p + "self_attn.out_proj.bias", VEC, L.bo, Hd);
-      params.add(p + "mlp.fc1.weight", PACKED, L.w1, static_cast<int64_t>(I) * Hd, I, Hd);
-      params.add(p + "mlp.fc1.bias", VEC, L.b1, I);
-      params.add(p + "mlp.fc2.weight", PACKED, L.w2, static_cast<int64_t>(Hd) * I, Hd, I);
-      params.add(p + "mlp.fc2.bias", VEC, L.b2, Hd);
-    }
+    enc.layout(arena, params, vm + "encoder.layers.", c.layers, Hd, I);
     post_g = arena.take<float>(Hd); post_b = arena.take<float>(Hd);
     params.add(vm + "post_layernorm.weight", VEC, post_g, Hd);
     params.add(vm + "post_layernorm.bias", VEC, post_b, Hd);
@@ -333,34 +302,10 @@ struct SafetyEngine {
     crop = arena.take<uint8_t>(mb * SAFETY_CROP * SAFETY_CROP * 3);
   }
 
-  int linear(const __half* A, int64_t T, int Kd, const __half* w, int N, const float* bias, const __half* resid,
-             __half* out, const std::string& tag, OpList& ops) {
-    GemmDesc d;
-    d.A = A; d.C = Kd; d.W = static_cast<int>(T); d.H = 1; d.B = 1; d.sW = Kd;
-    d.Wt = w; d.N = N; d.bias = bias; d.resid = resid; d.ldr = N; d.out = out; d.ldc = N;
-    return add_gemm(d, tag, ops);
-  }
-  int add_gemm(const GemmDesc& d, const std::string& tag, OpList& ops) {
-    auto L = std::make_shared<GemmLaunch>();
-    if (int e = plan_gemm(d, L.get())) {
-      set_error(tag + ": " + last_error());
-      return e;
-    }
-    ops.ops.push_back([L](cudaStream_t st, int) { return launch_gemm(*L, st); });
-    ops.tags.push_back(tag);
-    ops.launches += 1;
-    return 0;
-  }
-  void add(OpList& ops, const std::string& tag, OpFn f) {
-    ops.ops.push_back(std::move(f));
-    ops.tags.push_back(tag);
-    ops.launches += 1;
-  }
-
   // patch GEMM .. image embeddings for a chunk of B images whose patch rows and class tokens are in place
   int build_tower(int B, SafetyTower& t) {
     const sdw_safety_config& c = cfg;
-    const int Hd = c.hidden, I = c.intermediate;
+    const int Hd = c.hidden;
     const int64_t T = static_cast<int64_t>(B) * ntok;
     OpList& ops = t.ops;
     ops.clear();
@@ -371,51 +316,20 @@ struct SafetyEngine {
       d.out = x0 + Hd; d.o_sW = Hd; d.o_sB = static_cast<int64_t>(ntok) * Hd;
       d.resid = pos + Hd; d.r_sW = Hd; d.r_sB = 0;
       d.et = 1;  // the residual's batch stride 0 is not a tensor-map view
-      if (int e = add_gemm(d, "patch embedding " + std::to_string(K) + "->" + std::to_string(Hd) + " + pos", ops)) return e;
+      if (int e = ops.add_gemm(d, "patch embedding " + std::to_string(K) + "->" + std::to_string(Hd) + " + pos")) return e;
     }
     const float eps = c.eps;
-    __half *x = x1, *y = x0;
-    add(ops, "pre_layrnorm", [=](cudaStream_t st, int) { return layernorm(x0, Hd, T, Hd, pre_g, pre_b, eps, x1, Hd, st); });
-    for (int i = 0; i < c.layers; ++i) {
-      const SafetyLayer& L = layers[i];
-      const std::string p = "layer " + std::to_string(i) + " ";
-      __half* hh = h;
-      add(ops, p + "ln1", [=](cudaStream_t st, int) { return layernorm(x, Hd, T, Hd, L.ln1_g, L.ln1_b, eps, hh, Hd, st); });
-      {
-        GemmDesc g;
-        g.A = h; g.C = Hd; g.W = static_cast<int>(T); g.H = 1; g.B = 1; g.sW = Hd;
-        g.Wt = L.wqkv; g.N = 3 * Hd; g.bias = L.bqkv;
-        g.out = qk; g.ldc = 2 * Hd;
-        g.mode = GEMM_QKV_VT;
-        g.vt_col0 = 2 * Hd; g.vt_d = 64; g.vt_heads = c.heads; g.vt_ntok = ntok; g.vt = vt; g.vt_ld = vt_ld;
-        if (int e = add_gemm(g, p + "qkv + V^T", ops)) return e;
-      }
-      {
-        AttnDesc ad;
-        ad.q = qk; ad.q_ld = 2 * Hd; ad.k = qk + Hd; ad.k_ld = 2 * Hd; ad.vt = vt; ad.vt_ld = vt_ld;
-        ad.B = B; ad.Nq = ntok; ad.Nk = ntok; ad.heads = c.heads; ad.d = 64;
-        ad.out = h; ad.out_ld = Hd;
-        auto AL = std::make_shared<AttnLaunch>();
-        if (int e = plan_attention(ad, AL.get())) return e;
-        add(ops, p + "attention", [AL](cudaStream_t st, int) { return launch_attention(*AL, st); });
-      }
-      if (int e = linear(h, T, Hd, L.wo, Hd, L.bo, x, y, p + "out_proj + x", ops)) return e;
-      std::swap(x, y);
-      add(ops, p + "ln2", [=](cudaStream_t st, int) { return layernorm(x, Hd, T, Hd, L.ln2_g, L.ln2_b, eps, hh, Hd, st); });
-      if (int e = linear(h, T, Hd, L.w1, I, L.b1, nullptr, ff, p + "fc1", ops)) return e;
-      __half* f = ff;
-      const int act = c.act;
-      add(ops, p + "act", [=](cudaStream_t st, int) { return sdw_clip_act(f, T * I, act, st); });
-      if (int e = linear(ff, T, I, L.w2, Hd, L.b2, x, y, p + "fc2 + x", ops)) return e;
-      std::swap(x, y);
-    }
+    ops.add("pre_layrnorm", [=](cudaStream_t st, int) { return layernorm(x0, Hd, T, Hd, pre_g, pre_b, eps, x1, Hd, st); });
+    ClipEncoder::Buffers b;
+    b.x = x1; b.y = x0; b.h = h; b.ff = ff; b.qkv = qk; b.vt = vt; b.vt_ld = vt_ld;
+    if (int e = enc.emit(ops, B, ntok, eps, c.act, false, b)) return e;
     const int P = c.proj_dim;
     __half* pl = pooled;
     float *p32 = pooled32, *emb = embeds;
-    add(ops, "post_layernorm (CLS)", [=](cudaStream_t st, int) {
-      return layernorm(x, static_cast<int64_t>(ntok) * Hd, B, Hd, post_g, post_b, eps, pl, Hd, st);
+    ops.add("post_layernorm (CLS)", [=](cudaStream_t st, int) {  // the encoder's result is in x1
+      return layernorm(x1, static_cast<int64_t>(ntok) * Hd, B, Hd, post_g, post_b, eps, pl, Hd, st);
     });
-    add(ops, "visual_projection (fp32)", [=](cudaStream_t st, int) {
+    ops.add("visual_projection (fp32)", [=](cudaStream_t st, int) {
       if (int rc = half_to_float(pl, p32, static_cast<int64_t>(B) * Hd, 0, 1.f, st)) return rc;
       return linear_f32(p32, Hd, proj_w, nullptr, B, P, Hd, 0, 0, emb, P, st);
     });
@@ -652,13 +566,12 @@ int sdw_safety_debug_profile(sdw_safety* e, const uint8_t* frames_u8, int B, int
   SafetyTower* t = E->tower(B);
   if (!t) return 1;
   OpList ops;
-  ops.ops.push_back([=](cudaStream_t st, int) { return E->preprocess(frames_u8, B, H, W, nullptr, st); });
-  ops.tags.push_back("preprocess (resize, crop, normalise, patch rows)");
-  ops.ops.insert(ops.ops.end(), t->ops.ops.begin(), t->ops.ops.end());
-  ops.tags.insert(ops.tags.end(), t->ops.tags.begin(), t->ops.tags.end());
+  ops.add("preprocess (resize, crop, normalise, patch rows)",
+          [=](cudaStream_t st, int) { return E->preprocess(frames_u8, B, H, W, nullptr, st); });
+  ops.append(t->ops);
   int32_t* flags = reinterpret_cast<int32_t*>(E->pooled32);  // dead after the projection
-  ops.ops.push_back([=](cudaStream_t st, int) { return E->scores(E->embeds, B, flags, nullptr, nullptr, nullptr, 0, st); });
-  ops.tags.push_back("concept scores");
+  ops.add("concept scores",
+          [=](cudaStream_t st, int) { return E->scores(E->embeds, B, flags, nullptr, nullptr, nullptr, 0, st); });
   FILE* f = std::fopen(path, "w");
   SDW_REQUIRE(f, "cannot open the profile file");
   int rc = profile_ops(f, "safety", ops, static_cast<cudaStream_t>(stream), 0);

@@ -1,12 +1,18 @@
-"""The parameter table every native engine (sampler, CLIP text tower, upsampler) shares: its keys and element counts are
-the published checkpoint tables, nothing is loaded after bind, and load_param rejects what it cannot load with a
-message naming the parameter, before launching anything.  Plan-only binds to a fake aligned arena; no GPU."""
+"""The parameter table every native engine (sampler, CLIP text tower, upsampler, safety checker) shares: its keys and
+element counts are the published checkpoint tables, nothing is loaded after bind, and load_param rejects what it cannot
+load with a message naming the parameter, before launching anything.  Plan-only binds to a fake aligned arena; no
+GPU."""
 import ctypes as C
 import math
 
 import pytest
 
-ENGINES = ["engine", "clip", "upsampler"]
+ENGINES = ["engine", "clip", "upsampler", "safety"]
+# transformers' position_ids buffers, which are not parameters
+POSITION_IDS = {"clip": "text_model.embeddings.position_ids",
+                "safety": "vision_model.vision_model.embeddings.position_ids"}
+CHECKER_EXTRA = {"visual_projection.weight": 768 * 1024, "concept_embeds": 17 * 768, "special_care_embeds": 3 * 768,
+                 "concept_embeds_weights": 17, "special_care_embeds_weights": 3}
 
 
 def _config_and_table(prefix):
@@ -30,6 +36,18 @@ def _config_and_table(prefix):
         cfg = ClipConfig(kw["vocab_size"], kw["max_position_embeddings"], kw["hidden_size"], kw["num_hidden_layers"],
                          kw["num_attention_heads"], kw["intermediate_size"], 0, 1e-5, 2)
         return cfg, {k: t.numel() for k, t in sd.items() if not k.endswith("position_ids")}
+    if prefix == "safety":
+        import _safety_oracle as so
+        from transformers import CLIPVisionConfig, CLIPVisionModel
+
+        from stable_diffusion_videos_b200.safety import CLIP_MEAN, CLIP_STD, SafetyConfig
+
+        sd = CLIPVisionModel(CLIPVisionConfig(**so.VISION["ViT-L/14"])).state_dict()
+        want = {"vision_model." + k: t.numel() for k, t in sd.items() if not k.endswith("position_ids")}
+        want.update(CHECKER_EXTRA)
+        cfg = SafetyConfig(1024, 24, 16, 4096, 224, 14, 768, 17, 3, 1e-5, 2, 0, (C.c_float * 3)(*CLIP_MEAN),
+                           (C.c_float * 3)(*CLIP_STD))
+        return cfg, want
     from stable_diffusion_videos_b200.configs import esrgan_param_shapes
     from stable_diffusion_videos_b200.upsampling import UpsamplerConfig
 
@@ -80,6 +98,8 @@ def test_registry_is_the_published_key_table(engine):
         assert list(got) == list(want)  # esrgan_param_shapes's order
     if prefix == "engine":  # registration order, not alphabetical
         assert list(got)[:2] == ["time_embedding.linear_1.weight", "time_embedding.linear_1.bias"]
+    if prefix == "safety":  # the class embedding first, as CLIPVisionModel lists it
+        assert list(got)[0] == next(iter(want))
     assert fn("param_info")(bound, len(want), None, None) == 1
     assert b"index" in lib.sdw_last_error()
 
@@ -103,6 +123,10 @@ def test_load_param_rejects_before_launching(engine):
     assert b"not bound" in lib.sdw_last_error() and name.encode() in lib.sdw_last_error()
     assert fn("load_param")(bound, b"no.such.weight", src, C.c_int64(numel), None) == 1
     assert lib.sdw_last_error().endswith(b"unknown parameter: no.such.weight")
+    if prefix in POSITION_IDS:
+        key = POSITION_IDS[prefix].encode()
+        assert fn("load_param")(bound, key, src, C.c_int64(numel), None) == 1
+        assert lib.sdw_last_error().endswith(b"unknown parameter: " + key)
     assert fn("load_param")(bound, name.encode(), src, C.c_int64(numel + 1), None) == 1
     msg = f"parameter size mismatch for {name}: expected {numel}, got {numel + 1}"
     assert lib.sdw_last_error().decode().endswith(msg)

@@ -1,6 +1,6 @@
-"""The safety checker without a GPU: the native parameter registry against a diffusers-layout checker state dict built
-from transformers (plan-only bind), the fp64 restatement (tests/_safety_oracle.py) against transformers'
-CLIPVisionModel and CLIPImageProcessorPil, and the configuration checks that raise before anything is loaded."""
+"""The safety checker without a GPU: the fp64 restatement (tests/_safety_oracle.py) against transformers'
+CLIPVisionModel and CLIPImageProcessorPil, and the configuration checks that raise before anything is loaded.  Its
+native parameter registry is tested with the other engines' in test_params_cpu.py."""
 import ctypes as C
 import json
 
@@ -9,67 +9,6 @@ import pytest
 import torch
 
 import _safety_oracle as so
-
-CHECKER_EXTRA = {"visual_projection.weight": 768 * 1024, "concept_embeds": 17 * 768, "special_care_embeds": 3 * 768,
-                 "concept_embeds_weights": 17, "special_care_embeds_weights": 3}
-
-
-@pytest.fixture
-def registry():
-    from transformers import CLIPVisionConfig, CLIPVisionModel
-
-    from stable_diffusion_videos_b200 import _native
-    from stable_diffusion_videos_b200.safety import CLIP_MEAN, CLIP_STD, SafetyConfig
-
-    lib = _native.lib()
-    lib.sdw_safety_destroy.restype = None
-    kw = so.VISION["ViT-L/14"]
-    sd = CLIPVisionModel(CLIPVisionConfig(**kw)).state_dict()
-    want = {"vision_model." + k: t.numel() for k, t in sd.items() if not k.endswith("position_ids")}
-    want.update(CHECKER_EXTRA)
-    cfg = SafetyConfig(1024, 24, 16, 4096, 224, 14, 768, 17, 3, 1e-5, 2, 0, (C.c_float * 3)(*CLIP_MEAN),
-                       (C.c_float * 3)(*CLIP_STD))
-    h = C.c_void_p()
-    _native.check(lib.sdw_safety_create(C.byref(cfg), C.byref(h)))
-    n = C.c_uint64()
-    _native.check(lib.sdw_safety_arena_bytes(h, C.byref(n)))
-    lib.sdw_debug_plan_only(1)
-    try:
-        _native.check(lib.sdw_safety_bind(h, C.c_void_p(1 << 40), n))  # fake, aligned, never dereferenced
-        yield lib, h, want, sd
-    finally:
-        lib.sdw_debug_plan_only(0)
-        lib.sdw_safety_destroy(h)
-
-
-def test_registry_is_the_checker_key_table(registry):
-    lib, h, want, sd = registry
-    name, numel, got = C.c_char_p(), C.c_int64(), {}
-    for i in range(lib.sdw_safety_num_params(h)):
-        assert lib.sdw_safety_param_info(h, i, C.byref(name), C.byref(numel)) == 0
-        got[name.value.decode()] = numel.value
-    assert got == want
-    tower = {k: v for k, v in want.items() if k.startswith("vision_model.")}
-    assert sum(t.numel() for k, t in sd.items() if not k.endswith("position_ids")) == sum(tower.values())
-    assert len(got) == len(tower) + 5 and sum(got.values()) == sum(tower.values()) + sum(CHECKER_EXTRA.values())
-    assert not any(k.endswith("position_ids") for k in got)
-
-
-def test_nothing_loaded_and_bad_loads_rejected(registry):
-    lib, h, want, _ = registry
-    first = C.c_char_p()
-    assert lib.sdw_safety_missing_params(h, C.byref(first)) == len(want)
-    assert first.value.decode() == next(iter(want))
-    src = C.c_void_p(1 << 30)
-    assert lib.sdw_safety_load_param(h, b"vision_model.vision_model.embeddings.position_ids", src, C.c_int64(257),
-                                     None) == 1
-    assert lib.sdw_last_error().endswith(b"unknown parameter: vision_model.vision_model.embeddings.position_ids")
-    assert lib.sdw_safety_load_param(h, b"concept_embeds", src, C.c_int64(17 * 768 + 1), None) == 1
-    assert lib.sdw_last_error().decode().endswith(
-        f"parameter size mismatch for concept_embeds: expected {17 * 768}, got {17 * 768 + 1}")
-    assert lib.sdw_safety_missing_params(h, None) == len(want)
-    assert lib.sdw_safety_missing_params(None, None) == -1
-
 
 @pytest.mark.parametrize("field,value", [("hidden", 1000), ("image_size", 336), ("patch", 15), ("n_concepts", 70),
                                          ("act", 2), ("max_batch", 0)])
