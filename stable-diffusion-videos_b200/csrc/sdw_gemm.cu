@@ -8,7 +8,8 @@
 //               issues 4 x wgmma m64nBNk16 per accumulator from the shared-memory ring (fp32 accumulators in registers,
 //               one wgmma group kept in flight), then runs the fused epilogue of the tile from its registers:
 //               alpha / bias / time-embedding row vector / SiLU / residual / GEGLU / per-head V^T scatter, fp16 out,
-//               either stored directly or staged per 32-column chunk in shared memory and written by TMA stores.
+//               stored directly (the TMA epilogue's residual arriving per 32-column chunk by TMA into shared
+//               memory) or, for GEGLU, staged per 32-column chunk in shared memory and written by TMA stores.
 //   warp 8    : TMA producer — per K block one 4-D box of the shifted NHWC activation tile (OOB halo = zero fill =
 //               conv padding) and the K-major weight tile(s), SWIZZLE_128B, into an nstages-deep ring.
 //
@@ -66,9 +67,11 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)
   const int r0 = 64 * wg;
   const int tx = x0 + (r0 & (p.bw - 1)), ty = y0 + ((r0 >> p.lg_bw) & (p.bh - 1)), tb = b0 + (r0 >> (p.lg_bw + p.lg_bh));
   const bool issuer = (threadIdx.x & 127) == 0;
-  // TMA epilogue with a residual: chunk k's [64 rows x 32 columns] residual arrives by TMA in output buffer k & 1 itself
-  // (each thread overwrites exactly the elements it reads), issued one chunk ahead — the first one before this
-  // accumulator's first chunk — once the TMA store that last used the buffer has read it
+  // TMA epilogue with a residual: chunk k's [64 rows x 32 columns] residual arrives by TMA in buffer k & 1, issued one
+  // chunk ahead — the first one before this accumulator's first chunk — once every thread of the warpgroup has read
+  // the buffer's previous residual chunk (the barrier at the start of each chunk).  Plain outputs leave from registers
+  // by direct stores: a TMA store would wait behind the operand loads queued on the same TMA unit, and the chunk loop
+  // behind it for its buffer.
   const bool tma_res = use_tma && p.resid != nullptr;
   const int nch = (min(BN, p.N - n_base) + 31) >> 5;
   auto res_issue = [&](int c, uint32_t k) {
@@ -77,10 +80,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)
       tma_load_4d(&p.mapRes, &res_full[k & 1], stage + (k & 1) * 4096, n_base + 32 * c, tx, ty, tb);
     }
   };
-  if (tma_res && p.mode == GEMM_PLAIN) {
-    if (issuer) bulk_wait_group_read<1>();
-    res_issue(0, chunk_count);
-  }
+  if (tma_res && p.mode == GEMM_PLAIN) res_issue(0, chunk_count);
 
   auto value = [&](float v, int n, int h) {
     float o = v * p.alpha;
@@ -96,15 +96,16 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)
     if constexpr (XE != 0) o = fmaf(p.res_scale, r, o);
     else o += r;
   };
-  // 2 x 2 values (rows h = 0 / 1, columns n, n + 1) of the plain path, residual added, stored or staged
-  auto plain_pair = [&](int j, int n, uint8_t* staged, int scol) {
+  // 2 x 2 values (rows h = 0 / 1, columns n, n + 1) of the plain path, residual added (from the TMA-loaded chunk
+  // res_buf, column scol, or from global memory), stored
+  auto plain_pair = [&](int j, int n, const uint8_t* res_buf, int scol) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float o0 = n < p.N ? value(acc[4 * j + 2 * h], n, h) : 0.f;
       float o1 = n + 1 < p.N ? value(acc[4 * j + 2 * h + 1], n + 1, h) : 0.f;
-      if (staged && tma_res) {
+      if (res_buf) {
         const float2 f =
-            __half22float2(*reinterpret_cast<const __half2*>(staged + (lrow0 + 8 * h) * 64 + scol * 2));
+            __half22float2(*reinterpret_cast<const __half2*>(res_buf + (lrow0 + 8 * h) * 64 + scol * 2));
         add_res(o0, f.x);
         add_res(o1, f.y);
       } else if (p.resid && R[h].ok) {
@@ -126,9 +127,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)
           }
         }
       }
-      if (staged) {
-        *reinterpret_cast<uint32_t*>(staged + (lrow0 + 8 * h) * 64 + scol * 2) = pack_h2(o0, o1);
-      } else if (R[h].ok) {
+      if (R[h].ok) {
         __half* dst = p.out + R[h].out_off + n;
         if (vec2 && n + 1 < p.N) {
           *reinterpret_cast<uint32_t*>(dst) = pack_h2(o0, o1);
@@ -157,8 +156,8 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)
       }
     }
   };
-  // staged chunk (two 4 KB buffers per warpgroup, alternating): wait until the TMA store that last read the buffer is
-  // done, fill it, hand it to the async proxy, store
+  // staged GEGLU chunk (two 4 KB buffers per warpgroup, alternating): wait until the TMA store that last read the
+  // buffer is done, fill it, hand it to the async proxy, store
   auto stage_begin = [&]() {
     if (issuer) bulk_wait_group_read<1>();
     asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
@@ -226,16 +225,16 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, float (&acc)
       for (int jj = 0; jj < 4; ++jj) vt_pair(4 * c + jj, n + 8 * jj + q2);
       continue;
     }
-    if (use_tma) {
-      uint8_t* buf = stage_begin();
-      if (tma_res) {
-        if (issuer && c + 1 < nch) bulk_wait_group_read<0>();  // the previous chunk's store has read the other buffer
-        res_issue(c + 1, chunk_count + 1);
-        mbar_wait(&res_full[chunk_count & 1], (chunk_count >> 1) & 1);
-      }
+    if (tma_res) {
+      // every thread is done with the other buffer (chunk k - 1's residual): generic reads before the async-proxy write
+      fence_proxy_async_smem();
+      asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+      res_issue(c + 1, chunk_count + 1);
+      const uint8_t* buf = stage + (chunk_count & 1) * 4096;
+      mbar_wait(&res_full[chunk_count & 1], (chunk_count >> 1) & 1);
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) plain_pair(4 * c + jj, n + 8 * jj + q2, buf, 8 * jj + q2);
-      stage_end(buf, n);
+      ++chunk_count;
     } else {
 #pragma unroll
       for (int jj = 0; jj < 4; ++jj) plain_pair(4 * c + jj, n + 8 * jj + q2, nullptr, 0);
@@ -425,7 +424,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_kernel(const __grid_cons
         gemm_epilogue<BN, XE>(p, acc[sub], n0 + sub * BN, R, lane, wg, lrow0, stage_buf, res_full + 2 * wg, x0, y0, b0,
                           chunk_count);
     }
-    if (p.epi_tma && (threadIdx.x & 127) == 0) bulk_wait_group<0>();  // every output chunk has reached global memory
+    if (p.epi_tma && (threadIdx.x & 127) == 0) bulk_wait_group<0>();  // every TMA-stored chunk has reached global memory
   }
 
   // no CTA of a pair may exit while its peer can still multicast into its shared memory or arrive on its barriers
@@ -629,7 +628,7 @@ int plan_gemm(const GemmDesc& d, GemmLaunch* L) {
   L->tr = reuse ? 1 : 0;
   const int CL = ver == 2 ? 2 : 1;
   const int nsm = sm_count();
-  // ---- epilogue flavour: output chunks staged in shared memory and written by TMA stores where the views allow ----
+  // ---- epilogue flavour: residual chunks loaded and GEGLU output chunks stored by TMA where the views allow ----
   const int ncols = d.mode == GEMM_GEGLU ? d.N / 2 : (d.mode == GEMM_QKV_VT ? d.vt_col0 : d.N);
   const int64_t osW = d.o_sW || d.o_sH || d.o_sB ? d.o_sW : d.ldc;
   const int64_t osH = d.o_sW || d.o_sH || d.o_sB ? d.o_sH : OW * d.ldc;
