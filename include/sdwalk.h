@@ -70,14 +70,40 @@ typedef struct sdw_step_coef {
   float next_in_scale; /* scale_model_input factor for the next UNet call */
   float push_e, push_x; /* what the history keeps: (1, 0) = the combined eps (PLMS / LMS); DPM-Solver++ keeps the data
                          * prediction x0 = s / alpha_t - (sigma_t / alpha_t) e */
+  float c_z;            /* coefficient on the step noise z_f (DDIM eta > 0: sigma_t; Euler ancestral: sigma_up); 0 for
+                         * the deterministic schedules, whose zero-initialised structs keep their meaning */
 } sdw_step_coef;
-/* update: e = u + g (c - u);  s = use_x_base ? x_base : x;  x' = c_x s + c_e[0] e + sum_j c_e[1+j] hist[hist_slot[j]];
- * covers PNDM/PLMS (warm-up, cur_sample step, 4-term Adams-Bashforth), DDIM eps / v-prediction (eta = 0), LMS, Euler
- * and DPM-Solver++(2M) (history of x0) exactly; coefficients are computed on the host in fp64 (see schedulers.py). */
+/* update: e = u + g (c - u);  s = use_x_base ? x_base : x;
+ *         x' = c_x s + c_e[0] e + sum_j c_e[1+j] hist[hist_slot[j]] + c_z z_f;
+ * covers PNDM/PLMS (warm-up, cur_sample step, 4-term Adams-Bashforth), DDIM eps / v-prediction (any eta), LMS, Euler,
+ * Euler ancestral and DPM-Solver++(2M) (history of x0) exactly; coefficients are computed on the host in fp64 (see
+ * schedulers.py).  When c_z == 0 the noise is not generated. */
 
+/* Step noise of the stochastic schedules, one entry per frame (24 bytes).  Z(k, s, i), for a 64-bit key k, scheduler
+ * step s and flat NCHW index i inside one frame's [C][H][W] latent (C H W a multiple of 4):
+ *   Philox4x32-10 with counter (i / 4, s, 0x5344574E, 0) and key (lo32(k), hi32(k)) -> words x0..x3;
+ *   u(b) = ((b >> 9) + 1/2) 2^-23 (exact in fp32, strictly inside (0, 1));
+ *   z[4g+0] = r cospi(2 u(x1)), z[4g+1] = r sinpi(2 u(x1)) with r = sqrt(-2 ln u(x0)); lanes 2, 3 likewise from x2, x3.
+ * Frame f's noise is z_f = w_a Z(key_a) + w_b Z(key_b); a term whose weight is exactly 0 is not evaluated.  The noise
+ * does not depend on the frame's position in the batch, on F or on the launch. */
+typedef struct sdw_frame_noise {
+  uint64_t key_a, key_b;
+  float w_a, w_b;
+} sdw_frame_noise;
+
+/* rejects c_z != 0 (rc 1): a stochastic step goes through sdw_cfg_sched_step_noise */
 int sdw_cfg_sched_step(const void* eps_nhwc, int has_uncond, float* x, float* x_base, float* hist,
                        const sdw_step_coef* coef, int F, int C, int H, int W, void* next_in, int next_in_cpad,
                        void* stream);
+/* the same step with the noise term: noise_dev device [F] table (read only when c_z != 0), step = s of Z(k, s, i) */
+int sdw_cfg_sched_step_noise(const void* eps_nhwc, int has_uncond, float* x, float* x_base, float* hist,
+                             const sdw_step_coef* coef, int F, int C, int H, int W, void* next_in, int next_in_cpad,
+                             const sdw_frame_noise* noise_dev, int step, void* stream);
+/* tests / tooling: out fp32 [F][C][H][W] = z_f of every frame at `step`, from the device function the step kernel uses */
+int sdw_step_noise(const sdw_frame_noise* noise_dev, int F, int C, int H, int W, int step, float* out, void* stream);
+/* tests / tooling: the Philox4x32-10 block of the noise; ctr_key device uint32 [n][6] = (counter x4, key x2),
+ * out device uint32 [n][4], 16-byte aligned */
+int sdw_philox4x32_10(const uint32_t* ctr_key, int n, uint32_t* out, void* stream);
 
 /* latents [F][C][H][W] (fp16/fp32) -> fp32 state * sigma and the first NHWC fp16 model input */
 int sdw_latents_init(const void* latents, int dtype_is_f16, float init_noise_sigma, float in_scale, float* x,
@@ -143,6 +169,10 @@ int sdw_engine_sample(sdw_engine* e, const float* latents_f32, const void* cond_
 /* per-sample negative prompts (P:318-358 with a list `negative_prompt`): n = frames makes `uncond_f16` of the sample calls
  * a [frames][tokens][D] batch, n = 1 (default) one embedding shared by all frames */
 int sdw_engine_set_uncond_batch(sdw_engine* e, int n);
+/* the [frames] step-noise table of the stochastic schedules: enqueues a device-to-device copy of `noise_dev` into the
+ * engine's arena on `stream`, so a captured graph replays with the new keys without re-capture.  Sampling with a
+ * schedule that has a step with c_z != 0 returns 1 until a table has been set after bind. */
+int sdw_engine_set_frame_noise(sdw_engine* e, const sdw_frame_noise* noise_dev, void* stream);
 int sdw_engine_launches(const sdw_engine* e, int* prologue, int* unet_per_step, int* vae);
 /* The same sampler in three segments, for per-step callbacks (stable_diffusion_pipeline.py:429-430): `begin` stages the
  * inputs and runs the prologue (context assembly, cross-attention K/V, first model input); `steps` runs denoise steps

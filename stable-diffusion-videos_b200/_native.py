@@ -23,7 +23,13 @@ class StepCoef(C.Structure):
         ("guidance", C.c_float), ("c_x", C.c_float), ("c_e", C.c_float * 5),
         ("hist_slot", C.c_int32 * 4), ("use_x_base", C.c_int32), ("save_x_base", C.c_int32),
         ("push_slot", C.c_int32), ("next_in_scale", C.c_float), ("push_e", C.c_float), ("push_x", C.c_float),
+        ("c_z", C.c_float),
     ]
+
+
+class FrameNoise(C.Structure):
+    """sdw_frame_noise: frame f's step noise is w_a Z(key_a) + w_b Z(key_b) (include/sdwalk.h)"""
+    _fields_ = [("key_a", C.c_uint64), ("key_b", C.c_uint64), ("w_a", C.c_float), ("w_b", C.c_float)]
 
 
 class GemmDesc(C.Structure):

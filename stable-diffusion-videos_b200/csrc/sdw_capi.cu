@@ -33,8 +33,27 @@ int sdw_slerp_lerp_batch(const void* lat_a, const void* lat_b, const void* emb_a
 int sdw_cfg_sched_step(const void* eps_nhwc, int has_uncond, float* x, float* x_base, float* hist,
                        const sdw_step_coef* coef, int F, int C, int H, int W, void* next_in, int next_in_cpad,
                        void* stream) {
+  SDW_REQUIRE(coef, "null pointer");
+  SDW_REQUIRE(coef->c_z == 0.f, "sdw_cfg_sched_step: c_z != 0 is a stochastic step; use sdw_cfg_sched_step_noise");
   return cfg_sched_step(static_cast<const float*>(eps_nhwc), has_uncond, x, x_base, hist, coef, F, C, H, W, next_in,
-                        next_in_cpad, static_cast<cudaStream_t>(stream));
+                        next_in_cpad, nullptr, 0, static_cast<cudaStream_t>(stream));
+}
+
+static_assert(sizeof(sdw_frame_noise) == 24 && sizeof(sdw_frame_noise) == sizeof(FrameNoise), "frame-noise layout");
+
+int sdw_cfg_sched_step_noise(const void* eps_nhwc, int has_uncond, float* x, float* x_base, float* hist,
+                             const sdw_step_coef* coef, int F, int C, int H, int W, void* next_in, int next_in_cpad,
+                             const sdw_frame_noise* noise_dev, int step, void* stream) {
+  return cfg_sched_step(static_cast<const float*>(eps_nhwc), has_uncond, x, x_base, hist, coef, F, C, H, W, next_in,
+                        next_in_cpad, noise_dev, step, static_cast<cudaStream_t>(stream));
+}
+
+int sdw_step_noise(const sdw_frame_noise* noise_dev, int F, int C, int H, int W, int step, float* out, void* stream) {
+  return step_noise(noise_dev, F, C, H, W, step, out, static_cast<cudaStream_t>(stream));
+}
+
+int sdw_philox4x32_10(const uint32_t* ctr_key, int n, uint32_t* out, void* stream) {
+  return philox(ctr_key, n, out, static_cast<cudaStream_t>(stream));
 }
 
 int sdw_latents_init(const void* latents, int dtype_is_f16, float init_noise_sigma, float in_scale, float* x,

@@ -117,6 +117,86 @@ int slerp_lerp_batch(const void* lat_a, const void* lat_b, const void* emb_a, co
 }
 
 // ---------------------------------------------------------------------------------------------
+// Step noise of the stochastic samplers (DDIM eta > 0, Euler ancestral): a pure function Z(key, step, i) of a 64-bit
+// key, the scheduler step and the element's flat NCHW index i inside ONE frame, so it depends neither on the launch
+// geometry nor on the frame's position in the batch.  Philox4x32-10 (Salmon et al., SC'11) on the counter
+// (i / 4, step, 'SDWN', 0) gives four 32-bit words per group of four elements; two Box-Muller pairs turn them into
+// four normals.  Frame f mixes two keys: z_f = w_a Z(key_a) + w_b Z(key_b), a zero-weight term not evaluated.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) {
+      k0 += 0x9E3779B9u;
+      k1 += 0xBB67AE85u;
+    }
+    const uint32_t lo0 = c.x * 0xD2511F53u, hi0 = __umulhi(c.x, 0xD2511F53u);
+    const uint32_t lo1 = c.z * 0xCD9E8D57u, hi1 = __umulhi(c.z, 0xCD9E8D57u);
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+  }
+  return c;
+}
+
+// (m + 1/2) 2^-23 for the top 23 bits m: exact in fp32 and strictly inside (0, 1) (2^-24 .. 1 - 2^-24)
+__device__ __forceinline__ float philox_uniform(uint32_t b) {
+  return (static_cast<float>(b >> 9) + 0.5f) * 1.1920928955078125e-07f;
+}
+
+__device__ __forceinline__ float philox_normal(uint64_t key, int step, int64_t i) {
+  const uint4 r = philox4x32_10(make_uint4(static_cast<uint32_t>(i >> 2), static_cast<uint32_t>(step), 0x5344574Eu, 0u),
+                                static_cast<uint32_t>(key), static_cast<uint32_t>(key >> 32));
+  const int lane = static_cast<int>(i & 3);
+  const float u0 = philox_uniform(lane < 2 ? r.x : r.z), u1 = philox_uniform(lane < 2 ? r.y : r.w);
+  const float rad = sqrtf(-2.f * logf(u0));
+  float s, c;
+  sincospif(2.f * u1, &s, &c);
+  return rad * ((lane & 1) ? s : c);
+}
+
+__device__ __forceinline__ float frame_noise(const FrameNoise& fn, int step, int64_t i) {
+  float z = 0.f;
+  if (fn.w_a != 0.f) z = fn.w_a * philox_normal(fn.key_a, step, i);
+  if (fn.w_b != 0.f) z = fmaf(fn.w_b, philox_normal(fn.key_b, step, i), z);
+  return z;
+}
+
+__global__ void philox_kernel(const uint32_t* __restrict__ in, int n, uint32_t* __restrict__ out) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  const uint32_t* a = in + 6 * static_cast<int64_t>(j);
+  reinterpret_cast<uint4*>(out)[j] = philox4x32_10(make_uint4(a[0], a[1], a[2], a[3]), a[4], a[5]);
+}
+
+int philox(const uint32_t* in, int n, uint32_t* out, cudaStream_t stream) {
+  SDW_REQUIRE(in && out && n >= 0, "bad arguments");
+  SDW_REQUIRE(reinterpret_cast<uintptr_t>(out) % 16 == 0, "out must be 16-byte aligned");
+  if (n == 0) return 0;
+  philox_kernel<<<(n + 255) / 256, 256, 0, stream>>>(in, n, out);
+  SDW_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+__global__ void step_noise_kernel(const FrameNoise* __restrict__ noise, int F, int64_t per_frame, int step,
+                                  float* __restrict__ out) {
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= F * per_frame) return;
+  const int f = static_cast<int>(i / per_frame);
+  out[i] = frame_noise(noise[f], step, i - f * per_frame);
+}
+
+int step_noise(const void* noise, int F, int C, int H, int W, int step, float* out, cudaStream_t stream) {
+  SDW_REQUIRE(noise && out, "null pointer");
+  SDW_REQUIRE(F > 0 && C > 0 && H > 0 && W > 0 && step >= 0, "bad sizes");
+  const int64_t per = static_cast<int64_t>(C) * H * W;
+  SDW_REQUIRE(per % 4 == 0 && per / 4 <= 0xFFFFFFFFll, "a frame's element count must be a multiple of 4 below 2^34");
+  const int64_t n = F * per;
+  step_noise_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(static_cast<const FrameNoise*>(noise), F,
+                                                                                 per, step, out);
+  SDW_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
 // CFG + scheduler step.  One thread per latent element (f, c, y, x); all arithmetic fp32.
 // ---------------------------------------------------------------------------------------------
 struct StepCoef {
@@ -125,11 +205,13 @@ struct StepCoef {
   int use_x_base, save_x_base, push_slot;
   float next_in_scale;
   float push_e, push_x;  // hist[push_slot] := push_e * e + push_x * sample   (eps history: 1, 0; DPM-Solver++ keeps x0)
+  float c_z;             // coefficient on the step noise z_f (0: deterministic, the noise is not generated)
 };
 
 __global__ void cfg_sched_step_kernel(const float* __restrict__ eps, int has_uncond, float* __restrict__ x,
                                       float* __restrict__ x_base, float* __restrict__ hist, StepCoef k, int F, int C,
-                                      int H, int W, __half* __restrict__ next_in, int cpad) {
+                                      int H, int W, __half* __restrict__ next_in, int cpad,
+                                      const FrameNoise* __restrict__ noise, int step) {
   const int64_t n = static_cast<int64_t>(F) * C * H * W;
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= n) return;
@@ -153,6 +235,10 @@ __global__ void cfg_sched_step_kernel(const float* __restrict__ eps, int has_unc
 #pragma unroll
   for (int j = 0; j < 4; ++j)
     if (k.c_e[j + 1] != 0.f) acc = fmaf(k.c_e[j + 1], hist[static_cast<int64_t>(k.hist_slot[j]) * n + i], acc);
+  if (k.c_z != 0.f) {
+    const int64_t per = static_cast<int64_t>(C) * H * W;
+    acc = fmaf(k.c_z, frame_noise(noise[f], step, i - f * per), acc);
+  }
   const float xn = fmaf(k.c_x, xs, acc);
   if (k.push_slot >= 0) hist[static_cast<int64_t>(k.push_slot) * n + i] = fmaf(k.push_x, xs, k.push_e * e);
   x[i] = xn;
@@ -164,17 +250,22 @@ __global__ void cfg_sched_step_kernel(const float* __restrict__ eps, int has_unc
 }
 
 int cfg_sched_step(const float* eps, int has_uncond, float* x, float* x_base, float* hist, const void* coef, int F,
-                   int C, int H, int W, void* next_in, int cpad, cudaStream_t stream) {
+                   int C, int H, int W, void* next_in, int cpad, const void* noise, int step, cudaStream_t stream) {
   SDW_REQUIRE(eps && x && x_base && hist && coef, "null pointer");
   SDW_REQUIRE(F > 0 && C > 0 && H > 0 && W > 0, "bad sizes");
   StepCoef k;
   memcpy(&k, coef, sizeof(k));
   for (int j = 0; j < 4; ++j) SDW_REQUIRE(k.hist_slot[j] >= 0 && k.hist_slot[j] < 4, "hist slot out of range");
   SDW_REQUIRE(k.push_slot < 4, "push slot out of range");
+  if (k.c_z != 0.f) {
+    SDW_REQUIRE(noise, "c_z != 0 needs the frame-noise table");
+    SDW_REQUIRE(step >= 0 && (static_cast<int64_t>(C) * H * W) % 4 == 0, "noise: bad step or a frame size not a multiple of 4");
+  }
   const int64_t n = static_cast<int64_t>(F) * C * H * W;
   const int threads = 256;
   cfg_sched_step_kernel<<<static_cast<unsigned>((n + threads - 1) / threads), threads, 0, stream>>>(
-      eps, has_uncond, x, x_base, hist, k, F, C, H, W, static_cast<__half*>(next_in), cpad);
+      eps, has_uncond, x, x_base, hist, k, F, C, H, W, static_cast<__half*>(next_in), cpad,
+      static_cast<const FrameNoise*>(noise), step);
   SDW_CUDA_OK(cudaGetLastError());
   return 0;
 }

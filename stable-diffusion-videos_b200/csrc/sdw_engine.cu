@@ -86,6 +86,9 @@ struct Engine {
   __half* uncond_stage = nullptr;
   int uncond_batch = 1;  // 1: one unconditional embedding shared by all frames; frames: one per frame (per-sample negative prompts)
   void* lat_stage = nullptr;    // [F][4][H][W] fp32-sized
+  FrameNoise* noise = nullptr;  // [F] step-noise keys / weights of the stochastic schedules
+  bool noise_set = false;       // a table has been copied in since bind
+  bool stochastic = false;      // the schedule has a step with c_z != 0
   uint8_t* out_u8 = nullptr;    // [F][8H][8W][3]
   float* out_img_f32 = nullptr; // pre-clamp decoder output (debug / parity)
   float2* gn_ws = nullptr;
@@ -776,6 +779,7 @@ struct Engine {
     x_base = static_cast<float*>(arena.take(nlat * 4));
     hist = static_cast<float*>(arena.take(nlat * 4 * 4));
     lat_stage = arena.take(nlat * 4);
+    noise = static_cast<FrameNoise*>(arena.take(static_cast<size_t>(F) * sizeof(FrameNoise)));
     const int64_t per = static_cast<int64_t>(cfg.ctx_tokens) * cfg.cross_attention_dim;
     ctx = static_cast<__half*>(arena.take(static_cast<size_t>(Bn) * per * 2));
     cond_stage = static_cast<__half*>(arena.take(static_cast<size_t>(Bn) * per * 2));  // room for a full [Bn] context
@@ -901,6 +905,7 @@ int sdw_engine_bind(sdw_engine* e, void* arena, uint64_t bytes) {
   SDW_REQUIRE(reinterpret_cast<uintptr_t>(arena) % 1024 == 0, "arena must be 1024-byte aligned");
   if (int err = gemm_init()) return err;
   E->graph.reset();
+  E->noise_set = false;
   return E->build(false, arena);
 }
 
@@ -929,6 +934,8 @@ int sdw_engine_set_schedule(sdw_engine* e, int n_steps, const float* timesteps, 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   E->n_steps = n_steps;
   E->coefs.assign(coefs, coefs + n_steps);
+  E->stochastic = false;
+  for (const sdw_step_coef& k : E->coefs) E->stochastic |= k.c_z != 0.f;
   E->init_sigma = init_noise_sigma;
   E->first_in_scale = first_in_scale;
   E->graph.reset();
@@ -955,7 +962,7 @@ static int run_all(Engine* E, cudaStream_t st) {
   for (int s = 0; s < E->n_steps; ++s) {
     if (int rc = E->unet_ops.run(st, s)) return rc;
     if (int rc = cfg_sched_step(E->eps, c.guidance, E->x, E->x_base, E->hist, &E->coefs[s], F, lc, H, W,
-                                s + 1 < E->n_steps ? E->model_in : nullptr, lc, st))
+                                s + 1 < E->n_steps ? E->model_in : nullptr, lc, E->noise, s, st))
       return rc;
   }
   return E->vae_ops.run(st, 0);
@@ -990,6 +997,7 @@ int sdw_engine_sample(sdw_engine* e, const float* latents_f32, const void* cond_
   SDW_REQUIRE(E && latents_f32 && cond_f16 && out_u8, "null");
   SDW_REQUIRE(!E->dry && E->n_steps > 0, "engine not bound or schedule not set");
   SDW_REQUIRE(!E->cfg.guidance || uncond_f16, "guidance needs the unconditional embedding");
+  SDW_REQUIRE(!E->stochastic || E->noise_set, "stochastic schedule (c_z != 0) but no frame-noise table was set");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (int rc = stage_inputs(E, latents_f32, cond_f16, uncond_f16, st)) return rc;
   if (use_graph) {
@@ -1009,6 +1017,7 @@ int sdw_engine_sample_begin(sdw_engine* e, const float* latents_f32, const void*
   SDW_REQUIRE(E && latents_f32 && cond_f16, "null");
   SDW_REQUIRE(!E->dry && E->n_steps > 0, "engine not bound or schedule not set");
   SDW_REQUIRE(!E->cfg.guidance || uncond_f16, "guidance needs the unconditional embedding");
+  SDW_REQUIRE(!E->stochastic || E->noise_set, "stochastic schedule (c_z != 0) but no frame-noise table was set");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const sdw_engine_config& c = E->cfg;
   if (int rc = stage_inputs(E, latents_f32, cond_f16, uncond_f16, st)) return rc;
@@ -1023,12 +1032,14 @@ int sdw_engine_sample_steps(sdw_engine* e, int s0, int s1, float* out_latents, v
   Engine* E = reinterpret_cast<Engine*>(e);
   SDW_REQUIRE(E && !E->dry && E->n_steps > 0, "engine not bound or schedule not set");
   SDW_REQUIRE(0 <= s0 && s0 <= s1 && s1 <= E->n_steps, "step range out of the schedule");
+  SDW_REQUIRE(!E->stochastic || E->noise_set, "stochastic schedule (c_z != 0) but no frame-noise table was set");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const sdw_engine_config& c = E->cfg;
   for (int s = s0; s < s1; ++s) {
     if (int rc = E->unet_ops.run(st, s)) return rc;
     if (int rc = cfg_sched_step(E->eps, c.guidance, E->x, E->x_base, E->hist, &E->coefs[s], c.frames, c.in_channels,
-                                c.latent_h, c.latent_w, s + 1 < E->n_steps ? E->model_in : nullptr, c.in_channels, st))
+                                c.latent_h, c.latent_w, s + 1 < E->n_steps ? E->model_in : nullptr, c.in_channels,
+                                E->noise, s, st))
       return rc;
   }
   return copy_outputs(E, nullptr, out_latents, nullptr, st);
@@ -1048,6 +1059,16 @@ int sdw_engine_set_uncond_batch(sdw_engine* e, int n) {
   SDW_REQUIRE(n == 1 || n == E->cfg.frames, "the unconditional batch is 1 (shared) or `frames` (one per frame)");
   if (n != E->uncond_batch) E->graph.reset();  // the captured graph has the other addressing baked in
   E->uncond_batch = n;
+  return 0;
+}
+
+int sdw_engine_set_frame_noise(sdw_engine* e, const sdw_frame_noise* noise_dev, void* stream) {
+  Engine* E = reinterpret_cast<Engine*>(e);
+  SDW_REQUIRE(E && noise_dev, "null");
+  SDW_REQUIRE(!E->dry, "engine not bound");
+  SDW_CUDA_OK(cudaMemcpyAsync(E->noise, noise_dev, static_cast<size_t>(E->cfg.frames) * sizeof(FrameNoise),
+                              cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream)));
+  E->noise_set = true;
   return 0;
 }
 

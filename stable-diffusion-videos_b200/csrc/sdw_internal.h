@@ -225,8 +225,16 @@ void attention_plan_info(const AttnLaunch& L, int out[5]);
 int slerp_lerp_batch(const void* lat_a, const void* lat_b, const void* emb_a, const void* emb_b, const float* t,
                      int n_frames, int64_t n_lat, int64_t n_emb, int is_f16, float thr, void* out_lat, void* out_emb,
                      cudaStream_t stream);
+// layout of sdw_frame_noise (include/sdwalk.h): the two keys and weights of one frame's step noise
+struct FrameNoise {
+  uint64_t key_a, key_b;
+  float w_a, w_b;
+};
+// noise: device FrameNoise [F], read only when the step's c_z != 0
 int cfg_sched_step(const float* eps, int has_uncond, float* x, float* x_base, float* hist, const void* coef, int F,
-                   int C, int H, int W, void* next_in, int cpad, cudaStream_t stream);
+                   int C, int H, int W, void* next_in, int cpad, const void* noise, int step, cudaStream_t stream);
+int step_noise(const void* noise, int F, int C, int H, int W, int step, float* out, cudaStream_t stream);
+int philox(const uint32_t* in, int n, uint32_t* out, cudaStream_t stream);
 int latents_init(const void* latents, int is_f16, float sigma, float in_scale, float* x, void* model_in, int cpad,
                  int dup, int F, int C, int H, int W, cudaStream_t stream);
 int pack_weight(const void* w, int N, int C, int kh, int kw, int geglu, void* out, cudaStream_t stream);

@@ -63,7 +63,9 @@ class Engine:
         self._model = N.NativeModel("engine", c, 1024, self.device, "UNet / VAE")
         self._h = self._model.h
         self.n_steps = 0
+        self.stochastic = False
         self._plan_key = None
+        self._noise_dev = None
         # graph capture is illegal on the legacy default stream: the engine runs on its own stream, fenced both ways
         self._stream = torch.cuda.Stream(device=self.device)
 
@@ -92,9 +94,13 @@ class Engine:
                 raise N.SdwError(f"shape mismatch for {name}: {got} vs {want}")
         self._model.load(items, strict)
 
-    def set_scheduler(self, scheduler, num_inference_steps, guidance_scale):
+    def set_scheduler(self, scheduler, num_inference_steps, guidance_scale, eta=0.0):
+        """install the scheduler's plan; `eta` reaches the plan of the schedulers that take it (DDIM) and is ignored by
+        the others.  A plan with noise (c_z != 0 on some step) needs set_frame_noise before sampling."""
+        from .schedulers import accepts_eta
+
         scheduler.set_timesteps(num_inference_steps)
-        plan = scheduler.plan()
+        plan = scheduler.plan(eta=eta) if accepts_eta(scheduler) else scheduler.plan()
         n = len(plan)
         ts = np.asarray(scheduler.timesteps, dtype=np.float32)
         assert ts.shape[0] == n
@@ -110,13 +116,28 @@ class Engine:
             k.use_x_base, k.save_x_base, k.push_slot = st["use_x_base"], st["save_x_base"], st["push_slot"]
             k.next_in_scale = float(plan[i + 1]["in_scale"]) if i + 1 < n else 1.0
             k.push_e, k.push_x = float(st.get("push_e", 1.0)), float(st.get("push_x", 0.0))
+            k.c_z = float(st.get("c_z", 0.0))
         with torch.cuda.device(self.device):
             N.check(N.lib().sdw_engine_set_schedule(
                 self._h, n, ts.ctypes.data_as(C.POINTER(C.c_float)), coefs, C.c_float(scheduler.init_noise_sigma),
                 C.c_float(plan[0]["in_scale"]), N.stream_ptr()))
             torch.cuda.current_stream().synchronize()
         self.n_steps = n
+        self.stochastic = any(coefs[i].c_z != 0.0 for i in range(n))
         self._timesteps = [torch.tensor(t) for t in np.asarray(scheduler.timesteps).tolist()]
+
+    def set_frame_noise(self, table):
+        """the [frames] step-noise table (ctypes array of _native.FrameNoise, see noise.py) of the next sample calls;
+        copied into the engine on its stream, so a captured graph replays with it"""
+        if len(table) != self.frames:
+            raise ValueError(f"frame-noise table has {len(table)} entries, the engine samples {self.frames} frames")
+        from .noise import to_device
+
+        with torch.cuda.device(self.device):
+            self._stream.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(self._stream):
+                self._noise_dev = to_device(table, self.device)  # stays alive until the next table is set
+                N.check(N.lib().sdw_engine_set_frame_noise(self._h, N.ptr(self._noise_dev), N.stream_ptr()))
 
     def launches(self):
         a, b, c = C.c_int(), C.c_int(), C.c_int()

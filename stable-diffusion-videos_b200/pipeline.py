@@ -21,7 +21,8 @@ import torch
 from . import _native
 from .configs import UNetConfig, VAEConfig, random_state_dict, unet_param_shapes, vae_param_shapes
 from .engine import Engine
-from .schedulers import SCHEDULERS, PNDMScheduler
+from . import noise as _noise
+from .schedulers import SCHEDULERS, accepts_eta, check_eta
 
 
 class StableDiffusionPipelineOutput(dict):
@@ -241,9 +242,10 @@ class StableDiffusionWalkPipeline:
         kinds = {"PNDMScheduler": "pndm", "DDIMScheduler": "ddim", "LMSDiscreteScheduler": "lms",
                  "EulerDiscreteScheduler": "euler", "DPMSolverMultistepScheduler": "dpm"}
         if sc["_class_name"] not in kinds:
-            raise NotImplementedError(f"scheduler {sc['_class_name']} has no native plan (deterministic linear multistep "
-                                      f"rules only: {sorted(kinds)}); stochastic samplers (Euler ancestral, "
-                                      "DPM-Solver SDE variants) are not implemented")
+            raise NotImplementedError(f"scheduler {sc['_class_name']} cannot be loaded from scheduler_config.json (supported: "
+                                      f"{sorted(kinds)}); Euler ancestral runs natively when assigned after loading, "
+                                      "`pipe.scheduler = EulerAncestralDiscreteScheduler(...)` (schedulers.py); "
+                                      "DPM-Solver SDE variants are not implemented")
         kind = kinds[sc["_class_name"]]
         # scheduler_config.json fields beyond the beta schedule: the reference itself forces steps_offset = 1 and
         # clip_sample = False on whatever the checkpoint says (P:85-110), so those are applied, not read; anything this
@@ -325,11 +327,12 @@ class StableDiffusionWalkPipeline:
             self._engines = {key: eng}  # one resident engine (each carries its own packed weights)
         return eng
 
-    def _plan_key(self, num_inference_steps, guidance_scale):
+    def _plan_key(self, num_inference_steps, guidance_scale, eta=0.0):
         """identity of the native coefficient plan + captured graph: scheduler instance AND its configuration"""
         sc = self.scheduler.config
         return (type(self.scheduler).__name__, id(self.scheduler), sc.num_train_timesteps, sc.beta_start, sc.beta_end,
-                sc.prediction_type, sc.steps_offset, int(num_inference_steps), float(guidance_scale))
+                sc.prediction_type, sc.steps_offset, int(num_inference_steps), float(guidance_scale),
+                float(eta) if accepts_eta(self.scheduler) else 0.0)
 
     def _uncond(self, uncond_tokens):
         key = tuple(uncond_tokens)
@@ -359,8 +362,7 @@ class StableDiffusionWalkPipeline:
         if (callback_steps is None) or (not isinstance(callback_steps, int) or callback_steps <= 0):
             raise ValueError(f"`callback_steps` has to be a positive integer but is {callback_steps} of type"
                              f" {type(callback_steps)}.")
-        if eta != 0.0 and not isinstance(self.scheduler, PNDMScheduler) and type(self.scheduler).__name__.startswith("DDIM"):
-            raise NotImplementedError("stochastic DDIM (eta > 0) is not implemented; eta = 0 is the reference default")
+        check_eta(self.scheduler, eta)
 
         prompt_given = text_embeddings is None
         if text_embeddings is None:
@@ -413,9 +415,12 @@ class StableDiffusionWalkPipeline:
             latents = latents.to(self.device)
 
         want_float = output_type != "pil"
+        eng = self._prepare(height // 8, width // 8, B, guidance_scale, num_inference_steps, eta)
+        if eng.stochastic:  # keys are drawn only for a stochastic schedule: deterministic calls consume the RNG as before
+            eng.set_frame_noise(_noise.call_table(_noise.draw_call_keys(B, generator, self.device)))
         frames_u8, raw = self._sample_device(latents, text_embeddings, uncond, height, width, num_inference_steps,
                                              guidance_scale, want_raw=want_float, callback=callback,
-                                             callback_steps=callback_steps)
+                                             callback_steps=callback_steps, eta=eta)
         has_nsfw = None
         if self.safety_checker is not None:  # P:440-447: flagged images become black
             flags = self.safety_checker.check_frames(frames_u8, blackout=True)
@@ -433,16 +438,22 @@ class StableDiffusionWalkPipeline:
             return (image, has_nsfw)
         return StableDiffusionPipelineOutput(images=image, nsfw_content_detected=has_nsfw)
 
+    def _prepare(self, h8, w8, B, guidance_scale, num_inference_steps, eta):
+        """the resident engine for this shape with the scheduler's plan installed"""
+        eng = self._engine(h8, w8, B, guidance_scale > 1.0)
+        plan_key = self._plan_key(num_inference_steps, guidance_scale, eta)
+        if eng._plan_key != plan_key:
+            eng.set_scheduler(self.scheduler, num_inference_steps, guidance_scale, eta=eta)
+            eng._plan_key = plan_key
+        return eng
+
     def _sample_device(self, latents, text_embeddings, uncond, height, width, num_inference_steps, guidance_scale,
-                       want_raw=False, callback=None, callback_steps=1):
+                       want_raw=False, callback=None, callback_steps=1, eta=0.0):
         """native hot path: set-up (P:394-401), loop (P:412-430), decode + post-process (P:432-438, 450).
+        A stochastic schedule samples with the frame-noise table last given to the engine.
         Returns (uint8 NHWC frames on the device, pre-clamp fp32 decoder output or None)."""
         B = latents.shape[0]
-        eng = self._engine(height // 8, width // 8, B, guidance_scale > 1.0)
-        plan_key = self._plan_key(num_inference_steps, guidance_scale)
-        if eng._plan_key != plan_key:
-            eng.set_scheduler(self.scheduler, num_inference_steps, guidance_scale)
-            eng._plan_key = plan_key
+        eng = self._prepare(height // 8, width // 8, B, guidance_scale, num_inference_steps, eta)
         res = eng.sample(latents, text_embeddings.to(self.device), uncond, use_graph=True, return_raw=want_raw,
                          callback=callback, callback_steps=callback_steps)
         return res if want_raw else (res, None)
@@ -492,8 +503,7 @@ class StableDiffusionWalkPipeline:
             self.upsampler.to(self.device)
         if height % 8 != 0 or width % 8 != 0:  # raised by __call__ in the reference (P:271-272)
             raise ValueError(f"`height` and `width` have to be divisible by 8 but are {height} and {width}.")
-        if eta != 0.0 and type(self.scheduler).__name__.startswith("DDIM"):
-            raise NotImplementedError("stochastic DDIM (eta > 0) is not implemented; eta = 0 is the reference default")
+        check_eta(self.scheduler, eta)
         from . import parallel
 
         rank, world = self._dist if self._dist is not None else (0, 1)
@@ -518,8 +528,12 @@ class StableDiffusionWalkPipeline:
                 pad = batch_size - nb
                 embeds_batch = torch.cat([embeds_batch, embeds_batch[-1:].expand(pad, -1, -1)])
                 noise_batch = torch.cat([noise_batch, noise_batch[-1:].expand(pad, -1, -1, -1)])
+            eng = self._prepare(h8, w8, batch_size, guidance_scale, num_inference_steps, eta)
+            if eng.stochastic:  # step noise of these frames: a function of (seed_a, seed_b, T) only
+                i0 = lo + batch_idx * batch_size
+                eng.set_frame_noise(_noise.pad_table(_noise.walk_table(Tk[i0:i0 + nb], seed_a, seed_b), batch_size))
             frames_u8, _ = self._sample_device(noise_batch, embeds_batch, uncond, height, width, num_inference_steps,
-                                               guidance_scale)
+                                               guidance_scale, eta=eta)
             if self.safety_checker is not None:  # flagged frames are saved black (and upsampled black, P:546-552)
                 self.safety_checker.check_frames(frames_u8[:nb], blackout=True)
             if upsample:  # each rank upsamples its own block before the gather

@@ -5,8 +5,10 @@ The reference drives a diffusers scheduler object through `set_timesteps`, `time
 deterministic (PNDM/PLMS — the SD-1.4 default, DDIM with eta = 0 — the SD-2.1 default, LMS —
 examples/make_music_video.py:15-17, Euler) is a LINEAR multistep rule, so here `set_timesteps` pre-computes, in fp64 on
 the host, one `sdw_step_coef` per step (include/sdwalk.h); the update itself runs in one fused fp32 CUDA kernel
-together with classifier-free guidance.  `beta_schedule="scaled_linear"`, `steps_offset=1`,
-`set_alpha_to_one=False`, `clip_sample=False` as the reference forces (stable_diffusion_pipeline.py:85-110).
+together with classifier-free guidance.  The stochastic members (DDIM with eta > 0, Euler ancestral) are the same rules
+plus `c_z` times fresh Gaussian noise, generated inside that kernel from per-frame keys (noise.py).
+`beta_schedule="scaled_linear"`, `steps_offset=1`, `set_alpha_to_one=False`, `clip_sample=False` as the reference forces
+(stable_diffusion_pipeline.py:85-110).
 """
 from types import SimpleNamespace
 
@@ -40,7 +42,8 @@ class _Base:
         self.timesteps = None
         self.num_inference_steps = None
 
-    # the native plan: list of dict(c_x, c_e[5], hist_slot[4], use_x_base, save_x_base, push_slot, in_scale)
+    # the native plan: list of dict(c_x, c_e[5], hist_slot[4], use_x_base, save_x_base, push_slot, in_scale), plus the
+    # optional push_e / push_x (history contents) and c_z (noise coefficient, 0 when absent)
     def plan(self):
         raise NotImplementedError
 
@@ -129,7 +132,16 @@ class DDIMScheduler(_Base):
         r = self.config.num_train_timesteps // n
         self.timesteps = ((np.arange(0, n) * r).round()[::-1].copy() + self.config.steps_offset).astype(np.int64)
 
-    def plan(self):
+    def plan(self, eta=0.0):
+        """diffusers' DDIM step with use_clipped_model_output=False:
+            sigma = eta sqrt((1 - a_p) / (1 - a_t) (1 - a_t / a_p)),  D = sqrt(1 - a_p - sigma^2)
+            epsilon      : c_x = sqrt(a_p / a_t),                  c_e = D - sqrt(a_p (1 - a_t) / a_t)
+            v_prediction : c_x = sqrt(a_p a_t) + D sqrt(1 - a_t),  c_e = D sqrt(a_t) - sqrt(a_p (1 - a_t))
+        and c_z = sigma on the step noise.  D^2 stays under the square roots so that eta = 0 gives the same floats as
+        the deterministic form."""
+        eta = float(eta)
+        if not 0.0 <= eta <= 1.0:
+            raise ValueError(f"DDIM eta must lie in [0, 1], got {eta}")
         n = self.num_inference_steps
         r = self.config.num_train_timesteps // n
         ac = self.alphas_cumprod
@@ -139,16 +151,18 @@ class DDIMScheduler(_Base):
             prev = t - r
             a_t = ac[t]
             a_p = ac[prev] if prev >= 0 else self.final_alpha_cumprod
+            sigma = eta * ((1 - a_p) / (1 - a_t) * (1 - a_t / a_p)) ** 0.5 if eta else 0.0
+            d2 = 1 - a_p - sigma * sigma
             if self.config.prediction_type == "epsilon":
                 cx = (a_p / a_t) ** 0.5
-                ce = (1 - a_p) ** 0.5 - (a_p * (1 - a_t) / a_t) ** 0.5
+                ce = d2 ** 0.5 - (a_p * (1 - a_t) / a_t) ** 0.5
             elif self.config.prediction_type == "v_prediction":
-                cx = (a_p * a_t) ** 0.5 + ((1 - a_p) * (1 - a_t)) ** 0.5
-                ce = ((1 - a_p) * a_t) ** 0.5 - (a_p * (1 - a_t)) ** 0.5
+                cx = (a_p * a_t) ** 0.5 + (d2 * (1 - a_t)) ** 0.5
+                ce = (d2 * a_t) ** 0.5 - (a_p * (1 - a_t)) ** 0.5
             else:
                 raise ValueError(self.config.prediction_type)
             steps.append(dict(c_x=cx, c_e=[ce, 0, 0, 0, 0], hist_slot=[0, 0, 0, 0], use_x_base=0, save_x_base=0,
-                              push_slot=-1, in_scale=1.0))
+                              push_slot=-1, in_scale=1.0, c_z=float(sigma)))
         return steps
 
 
@@ -249,6 +263,29 @@ class EulerDiscreteScheduler(_Base):
         return steps
 
 
+class EulerAncestralDiscreteScheduler(EulerDiscreteScheduler):
+    """Euler ancestral (Karras et al. 2022 with ancestral sampling; diffusers' EulerAncestralDiscreteScheduler): each step
+    goes to sigma_down with the Euler rule, then adds fresh noise of standard deviation sigma_up,
+        sigma_up = sqrt(sigma_next^2 (sigma^2 - sigma_next^2) / sigma^2),  sigma_down = sqrt(sigma_next^2 - sigma_up^2),
+    so x' = c_x x + c_e e + sigma_up z with Euler's coefficients at dt = sigma_down - sigma.  Same sigma table, timesteps,
+    init_noise_sigma and input scaling as Euler; sigma_up = 0 on the last step."""
+
+    def plan(self):
+        steps = []
+        for i in range(self.num_inference_steps):
+            s, s_next = float(self.sigmas[i]), float(self.sigmas[i + 1])
+            s_up = (s_next ** 2 * (s ** 2 - s_next ** 2) / s ** 2) ** 0.5
+            s_down = (s_next ** 2 - s_up ** 2) ** 0.5
+            dt = s_down - s
+            if self.config.prediction_type == "epsilon":
+                cx, ce = 1.0, dt
+            else:
+                cx, ce = 1.0 + dt * s / (s * s + 1.0), dt / (s * s + 1.0) ** 0.5
+            steps.append(dict(c_x=cx, c_e=[ce, 0, 0, 0, 0], hist_slot=[0, 0, 0, 0], use_x_base=0, save_x_base=0,
+                              push_slot=-1, in_scale=1.0 / (s * s + 1.0) ** 0.5, c_z=s_up))
+        return steps
+
+
 class DPMSolverMultistepScheduler(_Base):
     """DPM-Solver++ (2M), the diffusers default configuration (algorithm_type "dpmsolver++", solver_order 2,
     solver_type "midpoint", lower_order_final=True, no thresholding): a two-step linear multistep rule on the DATA
@@ -298,4 +335,18 @@ class DPMSolverMultistepScheduler(_Base):
         return steps
 
 
-SCHEDULERS = {"dpm": DPMSolverMultistepScheduler, "pndm": PNDMScheduler, "ddim": DDIMScheduler, "lms": LMSDiscreteScheduler, "euler": EulerDiscreteScheduler}
+SCHEDULERS = {"dpm": DPMSolverMultistepScheduler, "pndm": PNDMScheduler, "ddim": DDIMScheduler, "lms": LMSDiscreteScheduler,
+              "euler": EulerDiscreteScheduler, "euler_a": EulerAncestralDiscreteScheduler}
+
+
+def accepts_eta(scheduler):
+    """whether the scheduler's plan takes `eta` (DDIM), as the reference asks of `scheduler.step` (P:404-410)"""
+    import inspect
+
+    return "eta" in inspect.signature(scheduler.plan).parameters
+
+
+def check_eta(scheduler, eta):
+    """eta is a DDIM parameter in [0, 1]; the other schedulers ignore it, as in the reference"""
+    if accepts_eta(scheduler) and not 0.0 <= float(eta) <= 1.0:
+        raise ValueError(f"DDIM eta must lie in [0, 1], got {eta}")
